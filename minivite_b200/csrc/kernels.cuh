@@ -921,62 +921,134 @@ __global__ void __launch_bounds__(256) k_collect_heavy(int lnv, const uint32_t *
 // kernels compare the original ids kept as labels.
 // key = level << 22 | region  (atomicMin: lowest level wins, then lowest region -> deterministic)
 // ----------------------------------------------------------------------------------------------
-#ifndef MV_BFS_SUB
-#define MV_BFS_SUB 4
-#endif
 constexpr unsigned int kBfsRegionBits = 22;
 constexpr unsigned int kBfsUnreached = 0xFFFFFFFFu;
+// edges per lane whose loads are all issued before the first compare (BFS expansion and CSR permute); on H100 at
+// config 2, 16 beat 8 and 4 in both kernels (DESIGN.md §3.3)
+constexpr int kEdgeBatch = 16;
 
+// A warp owns 32 rows whose edges form one range; `off` is this lane's row start within it (rows past the end hold the
+// range's length).  Returns the row that edge j of the range belongs to: the last lane with off <= j.
+__device__ __forceinline__ int row_of_edge(uint32_t off, uint32_t j) {
+  int o = 0;
+#pragma unroll
+  for (int s = 16; s; s >>= 1)
+    if (__shfl_sync(0xffffffffu, off, o + s) <= j) o += s;
+  return o;
+}
+
+// Frontier-queue BFS.  queue[] holds the reached vertices in BFS order: level L is the segment [lo, hi), and
+// level_count[L] counts the vertices level L appends (zeroed here, read only after the barrier that ends level L,
+// so every CTA derives the same next segment).  A warp takes 32 frontier vertices, spreads their edges over its lanes
+// and issues kEdgeBatch loads per lane at each step before any compare.  The vertex whose atomicMin finds it
+// unreached appends it (once).  Only the order inside a level's segment depends on timing; keys do not (lowest level,
+// then lowest region).
+// Level bitmaps: lmap holds four bitmaps, interleaved per 32 vertices (one 16-byte word), bitmap l % 4 marking the
+// vertices of level l.  Expanding level L skips every neighbour marked in the bitmaps of levels L-1 and L, whose keys
+// are already below the new key, with a probe of the 8 MB lmap instead of the 64 MB key[] array; level L+1's claims
+// are marked in bitmap (L+1) % 4, and bitmap (L+2) % 4 (level L-2, no longer read) is cleared for level L+1's claims.
 __global__ void __launch_bounds__(256) k_msbfs(int lnv, const uint32_t *rowptr, const int32_t *tails, uint32_t *key,
-                                               int region_stride, int max_levels, unsigned int *level_flags) {
+                                               int region_stride, int max_levels, int32_t *queue,
+                                               unsigned int *level_count, uint32_t *lmap) {
   namespace cg = cooperative_groups;
   cg::grid_group grid = cg::this_grid();
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gsz = gridDim.x * blockDim.x;
-  for (int v = gtid; v < lnv; v += gsz)
-    key[v] = (v % region_stride == 0) ? (unsigned int)(v / region_stride) : kBfsUnreached;
+  const int nwords = (lnv + 31) >> 5;
+  for (int v = gtid; v < lnv; v += gsz) {
+    const bool seed = v % region_stride == 0;
+    key[v] = seed ? (unsigned int)(v / region_stride) : kBfsUnreached;
+    if (seed) queue[v / region_stride] = v;
+  }
+  for (int q = gtid; q < nwords; q += gsz) {          // the seeds are level 0
+    const long long end = min(32LL * q + 32, (long long)lnv);
+    unsigned int seeds = 0;
+    for (long long v = (32LL * q + region_stride - 1) / region_stride * region_stride; v < end; v += region_stride)
+      seeds |= 1u << (v & 31);
+    reinterpret_cast<uint4 *>(lmap)[q] = make_uint4(seeds, 0u, 0u, 0u);
+  }
+  for (int l = gtid; l < max_levels; l += gsz) level_count[l] = 0;
   grid.sync();
+  const unsigned int full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
-  // Every warp inspects 32 consecutive keys per step.  The frontier vertices it finds are parked in shared memory and
-  // expanded MV_BFS_SUB at a time, 32 / MV_BFS_SUB lanes each, so that several adjacency reads and their dependent
-  // key[] probes are in flight per warp (one vertex at a time, 32 lanes each, left two dependent memory round trips per
-  // frontier vertex exposed).
-  // The kernel is bound by the random 32-byte key[] sectors of the edge probes.  Two filters in front of the keys were
-  // measured and removed because the extra dependent load cost more than the sectors it saved: a bit per expanded
-  // vertex and a byte per vertex holding its level.
-  constexpr int kBfsSub = MV_BFS_SUB, kBfsLanes = 32 / kBfsSub;
-  __shared__ uint32_t s_front[256 / 32][32][3];
-  uint32_t(*front)[3] = s_front[threadIdx.x >> 5];
-  for (int level = 0; level < max_levels; level++) {
-    bool any = false;
-    for (int vb = (gtid - lane); vb < lnv; vb += gsz) {
-      const int v = vb + lane;
-      unsigned int k = kBfsUnreached;
-      if (v < lnv) k = __ldcg(key + v);
-      const bool active = (k != kBfsUnreached) && ((k >> kBfsRegionBits) == (unsigned int)level);
-      const unsigned int m = __ballot_sync(0xffffffffu, active);
-      if (m == 0) continue;
-      any = true;
-      if (active) {
-        const int slot = __popc(m & ((1u << lane) - 1u));
-        front[slot][0] = ((unsigned int)(level + 1) << kBfsRegionBits) | (k & ((1u << kBfsRegionBits) - 1));
-        front[slot][1] = rowptr[v];
-        front[slot][2] = rowptr[v + 1];
+  const unsigned int gwarp = gtid >> 5, nwarps = gsz >> 5;
+  unsigned int lo = 0, hi = (unsigned int)((lnv - 1) / region_stride + 1);
+  for (int level = 0; level < max_levels && lo < hi; level++) {
+    const unsigned int nk_level = (unsigned int)(level + 1) << kBfsRegionBits;
+    const int m_prev = (level + 3) & 3, m_cur = level & 3, m_next = (level + 1) & 3;
+    for (int q = gtid; q < nwords; q += gsz) lmap[4 * q + ((level + 2) & 3)] = 0u;
+    for (unsigned int c = lo + gwarp * 32u; c < hi; c += nwarps * 32u) {
+      uint32_t b = 0, d = 0, nk = 0;
+      if (c + lane < hi) {
+        const int v = __ldcg(queue + c + lane);                       // appended by other SMs: read through L2
+        nk = nk_level | (__ldcg(key + v) & ((1u << kBfsRegionBits) - 1));
+        b = rowptr[v];
+        d = rowptr[v + 1] - b;
       }
-      __syncwarp();
-      const int cnt = __popc(m);
-      for (int i = lane / kBfsLanes; i < cnt; i += kBfsSub) {
-        const unsigned int nk = front[i][0];
-        const uint32_t e1 = front[i][2];
-        for (uint32_t e = front[i][1] + (lane % kBfsLanes); e < e1; e += kBfsLanes) {
-          const int w = tails[e];
-          if (w < lnv && __ldcg(key + w) > nk) atomicMin(&key[w], nk);
+      uint32_t incl = d;
+#pragma unroll
+      for (int s = 1; s < 32; s <<= 1) {
+        const uint32_t y = __shfl_up_sync(full, incl, s);
+        if (lane >= s) incl += y;
+      }
+      const uint32_t off = incl - d, total = __shfl_sync(full, incl, 31);
+      for (uint32_t j0 = 0; j0 < total; j0 += 32 * kEdgeBatch) {
+        int w[kEdgeBatch];
+        uint32_t nkw[kEdgeBatch], kw[kEdgeBatch];
+#pragma unroll
+        for (int u = 0; u < kEdgeBatch; u++) {
+          const uint32_t j = j0 + u * 32 + lane;
+          const int o = row_of_edge(off, j);
+          const uint32_t e = __shfl_sync(full, b, o) + (j - __shfl_sync(full, off, o));
+          nkw[u] = __shfl_sync(full, nk, o);
+          w[u] = j < total ? tails[e] : lnv;                          // ghosts (w >= lnv) are never probed
+        }
+        uint32_t mp[kEdgeBatch], mc[kEdgeBatch];
+#pragma unroll
+        for (int u = 0; u < kEdgeBatch; u++) {
+          mp[u] = mc[u] = 0;
+          if (w[u] < lnv) {
+            mp[u] = __ldcg(lmap + 4 * (w[u] >> 5) + m_prev);
+            mc[u] = __ldcg(lmap + 4 * (w[u] >> 5) + m_cur);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < kEdgeBatch; u++)
+          if ((((mp[u] | mc[u]) >> (w[u] & 31)) & 1u)) w[u] = lnv;
+#pragma unroll
+        for (int u = 0; u < kEdgeBatch; u++) kw[u] = w[u] < lnv ? __ldcg(key + w[u]) : 0u;
+        unsigned int nnew = 0;
+#pragma unroll
+        for (int u = 0; u < kEdgeBatch; u++) {
+          bool claimed = false;
+          if (w[u] < lnv && kw[u] > nkw[u]) claimed = atomicMin(&key[w[u]], nkw[u]) == kBfsUnreached;
+          if (claimed) {
+            nnew++;
+            atomicOr(lmap + 4 * (w[u] >> 5) + m_next, 1u << (w[u] & 31));
+          } else {
+            w[u] = -1;
+          }
+        }
+        // warp-aggregated append: one atomic per warp and batch
+        unsigned int pos = nnew;
+#pragma unroll
+        for (int s = 1; s < 32; s <<= 1) {
+          const unsigned int y = __shfl_up_sync(full, pos, s);
+          if (lane >= s) pos += y;
+        }
+        const unsigned int cnt = __shfl_sync(full, pos, 31);
+        if (cnt) {
+          unsigned int base = 0;
+          if (lane == 31) base = atomicAdd(level_count + level, cnt);
+          pos = hi + __shfl_sync(full, base, 31) + pos - nnew;
+#pragma unroll
+          for (int u = 0; u < kEdgeBatch; u++)
+            if (w[u] >= 0) queue[pos++] = w[u];
         }
       }
-      __syncwarp();
     }
-    if (__syncthreads_or(any) && threadIdx.x == 0) level_flags[level] = 1;
     grid.sync();
-    if (__ldcg(level_flags + level) == 0) break;
+    lo = hi;
+    hi += __ldcg(level_count + level);
   }
 }
 
@@ -998,34 +1070,67 @@ __global__ void __launch_bounds__(256) k_bfs_sortkeys(int lnv, const uint32_t *k
   }
 }
 
-// perm[new] = old  ->  inv[old] = new, lab[new] = global original id
+// perm[new] = old  ->  inv[old] = new (unless inv is null), lab[new] = global original id, deg_new[new] = degree
 __global__ void __launch_bounds__(256) k_perm_inverse(int lnv, const int32_t *perm, long long base, int32_t *inv, int32_t *lab,
                                                       const uint32_t *rowptr_old, uint32_t *deg_new) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= lnv; i += gridDim.x * blockDim.x) {
     if (i == lnv) { deg_new[i] = 0; continue; }
     const int o = perm[i];
-    inv[o] = i;
+    if (inv) inv[o] = i;
     lab[i] = (int32_t)(base + o);
     deg_new[i] = rowptr_old[o + 1] - rowptr_old[o];
   }
 }
 
 // adjacency of new vertex i := adjacency of old vertex perm[i], tails renumbered (ghost slots unchanged),
-// edge order preserved (weighted sums keep the reference's summation order)
+// edge order preserved (weighted sums keep the reference's summation order).  A warp owns 32 consecutive new vertices,
+// whose rows are one contiguous range of the new CSR; it walks that range edge-parallel, kEdgeBatch edges per lane, so
+// the tails_old reads and then the inv[] gathers are issued kEdgeBatch at a time and the stores are coalesced.  Also
+// checks that every old adjacency list is in tails_ascend order (sets *unordered otherwise).
 __global__ void __launch_bounds__(256) k_permute_adj(int lnv, const int32_t *perm, const int32_t *inv, const uint32_t *rowptr_old,
                                                      const int32_t *tails_old, const double *w_old, const uint32_t *rowptr_new,
                                                      int32_t *tails_new, double *w_new, int nlow, unsigned int *unordered) {
-  const int lane = threadIdx.x & 7;
-  const int tile = (blockIdx.x * blockDim.x + threadIdx.x) >> 3, ntiles = (gridDim.x * blockDim.x) >> 3;
+  const unsigned int full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const long long gwarp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * (long long)blockDim.x) >> 5;
   bool bad = false;
-  for (int i = tile; i < lnv; i += ntiles) {
-    const int o = perm[i];
-    const uint32_t s0 = rowptr_old[o], s1 = rowptr_old[o + 1], d0 = rowptr_new[i];
-    for (uint32_t k = lane; k < s1 - s0; k += 8) {
-      const int t = tails_old[s0 + k];
-      if (k && !tails_ascend(tails_old[s0 + k - 1], t, lnv, nlow)) bad = true;   // neighbour lane's element: an L1 hit
-      tails_new[d0 + k] = (t < lnv) ? inv[t] : t;
-      if (w_old) w_new[d0 + k] = w_old[s0 + k];
+  for (long long i0 = gwarp * 32; i0 < lnv; i0 += nwarps * 32) {
+    const long long i = i0 + lane;
+    const uint32_t d0 = rowptr_new[i0], total = rowptr_new[min(i0 + 32, (long long)lnv)] - d0;
+    uint32_t off = total, s0 = 0;
+    if (i < lnv) {
+      off = rowptr_new[i] - d0;
+      s0 = rowptr_old[perm[i]];
+    }
+    int carry = 0;                                     // lane 31's tail of the previous batch
+    for (uint32_t j0 = 0; j0 < total; j0 += 32 * kEdgeBatch) {
+      int t[kEdgeBatch];
+      uint32_t k[kEdgeBatch];
+#pragma unroll
+      for (int u = 0; u < kEdgeBatch; u++) {
+        const uint32_t j = j0 + u * 32 + lane;
+        const int o = row_of_edge(off, j);
+        k[u] = j - __shfl_sync(full, off, o);          // position inside the row
+        const uint32_t src = __shfl_sync(full, s0, o) + k[u];
+        t[u] = 0;
+        if (j < total) {
+          t[u] = tails_old[src];
+          if (w_old) w_new[d0 + j] = w_old[src];
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < kEdgeBatch; u++) {
+        const int up = __shfl_up_sync(full, t[u], 1);
+        const int prev = lane ? up : carry;            // the row's previous edge whenever k > 0
+        carry = __shfl_sync(full, t[u], 31);
+        if (j0 + u * 32 + lane < total && k[u] && !tails_ascend(prev, t[u], lnv, nlow)) bad = true;
+      }
+      int n[kEdgeBatch];
+#pragma unroll
+      for (int u = 0; u < kEdgeBatch; u++) n[u] = (j0 + u * 32 + lane < total && t[u] < lnv) ? inv[t[u]] : t[u];
+#pragma unroll
+      for (int u = 0; u < kEdgeBatch; u++)
+        if (j0 + u * 32 + lane < total) tails_new[d0 + j0 + u * 32 + lane] = n[u];
     }
   }
   if (bad) *unordered = 1;

@@ -134,7 +134,7 @@ struct mvgpu_ctx {
   DevBuf<uint32_t> bfs_key, sortkey, sortkey2, deg_new, rowptr2;
   DevBuf<int32_t> ids, perm, inv, lab, tails2, final_orig;
   DevBuf<double> weights2;
-  DevBuf<unsigned int> level_flags;
+  DevBuf<unsigned int> bfs_level_count;
   bool reordered = false;
   int relabel = 0;
   double reorder_s = 0.0;
@@ -645,19 +645,21 @@ int setup_run(mvgpu_ctx *c) {
       cudaEvent_t r0 = get_event(c, 2), r1 = get_event(c, 3);
       CK(cudaEventRecord(r0, s));
       TRY(c->perm.ensure(lnv)); TRY(c->inv.ensure(lnv)); TRY(c->lab.ensure(lnv)); TRY(c->ids.ensure(lnv));
-      TRY(c->bfs_key.ensure(lnv)); TRY(c->sortkey.ensure(lnv)); TRY(c->sortkey2.ensure(lnv));
+      TRY(c->bfs_key.ensure(lnv)); TRY(c->sortkey.ensure(lnv)); TRY(c->sortkey2.ensure(std::max(lnv, 4 * ((lnv + 31) / 32))));
       TRY(c->deg_new.ensure(lnv + 1)); TRY(c->rowptr2.ensure(lnv + 1 + 40)); TRY(c->tails2.ensure(lne + 4));
       if (!c->unit) TRY(c->weights2.ensure(lne + 4));
       const int max_levels = 1023;
-      TRY(c->level_flags.ensure(max_levels + 1));
-      CK(cudaMemsetAsync(c->level_flags.p, 0, sizeof(unsigned int) * (max_levels + 1), s));
       if (want) {
+        TRY(c->bfs_level_count.ensure(max_levels));
         int occ = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_msbfs, 256, 0));
         if (occ < 1) return fail("k_msbfs cannot be made resident");
         int ilnv = (int)lnv, stride = c->opt_region, ml = max_levels;
-        const uint32_t *rp = src_rowptr; const int32_t *tl = src_tails; uint32_t *key = c->bfs_key.p; unsigned int *lf = c->level_flags.p;
-        void *args[] = {&ilnv, &rp, &tl, &key, &stride, &ml, &lf};
+        const uint32_t *rp = src_rowptr; const int32_t *tl = src_tails; uint32_t *key = c->bfs_key.p;
+        // the BFS queue and its level bitmaps (4 bits per vertex) live in ids and sortkey2, which k_bfs_sortkeys and the
+        // sort only write after the BFS
+        int32_t *q = c->ids.p; unsigned int *lc = c->bfs_level_count.p; uint32_t *lm = c->sortkey2.p;
+        void *args[] = {&ilnv, &rp, &tl, &key, &stride, &ml, &q, &lc, &lm};
         CK(cudaLaunchCooperativeKernel((void *)k_msbfs, dim3(occ * nsm), dim3(256), args, 0, s));
         // sort by (region, level): only the bits that can be set take part (one radix pass less than a 32-bit sort)
         const long long nregions = (lnv + stride - 1) / stride;
@@ -676,18 +678,28 @@ int setup_run(mvgpu_ctx *c) {
         k_bfs_sortkeys<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->bfs_key.p, c->sortkey.p, c->perm.p, 0xFFFFFFFFu);
         c->tm.kernel_launches++;
       }
-      k_perm_inverse<<<grid_for(lnv + 1, 256, nsm), 256, 0, s>>>((int)lnv, c->perm.p, c->base, c->inv.p, c->lab.p, src_rowptr, c->deg_new.p);
+      k_perm_inverse<<<grid_for(lnv + 1, 256, nsm), 256, 0, s>>>((int)lnv, c->perm.p, c->base, want ? nullptr : c->inv.p, c->lab.p, src_rowptr, c->deg_new.p);
       c->tm.kernel_launches++;
       if (want) {
+        // inv[old] = new as a second radix sort (keys perm, values the ids 0..lnv-1 still in c->ids): lnv random 4-byte
+        // stores inv[perm[i]] = i cost more than twice as much as the sort's bucketed scatters (DESIGN.md §3.3)
+        int bits = 1;
+        while ((1LL << bits) < lnv && bits < 31) bits++;
+        const uint32_t *pk = reinterpret_cast<const uint32_t *>(c->perm.p);
         size_t tb = 0;
+        cub::DeviceRadixSort::SortPairs(nullptr, tb, pk, c->sortkey2.p, c->ids.p, c->inv.p, (int)lnv, 0, bits, s);
+        TRY(c->cub_tmp.ensure(tb));
+        tb = c->cub_tmp.cap;
+        CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tb, pk, c->sortkey2.p, c->ids.p, c->inv.p, (int)lnv, 0, bits, s));
+        tb = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, tb, c->deg_new.p, c->rowptr2.p, (int)lnv + 1, s);
         TRY(c->cub_tmp.ensure(tb));
         tb = c->cub_tmp.cap;
         CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, c->deg_new.p, c->rowptr2.p, (int)lnv + 1, s));
-        k_permute_adj<<<grid_for(lnv * 8, 256, nsm, 16), 256, 0, s>>>((int)lnv, c->perm.p, c->inv.p, src_rowptr, src_tails, src_weights,
-                                                                    c->rowptr2.p, c->tails2.p, c->unit ? nullptr : c->weights2.p,
-                                                                    (int)c->roff[c->rank], &d_sc->unordered);
-        c->tm.kernel_launches += 2;
+        k_permute_adj<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->perm.p, c->inv.p, src_rowptr, src_tails, src_weights,
+                                                               c->rowptr2.p, c->tails2.p, c->unit ? nullptr : c->weights2.p,
+                                                               (int)c->roff[c->rank], &d_sc->unordered);
+        c->tm.kernel_launches += 3;
         src_rowptr = c->rowptr2.p;
         src_tails = c->tails2.p;
         src_weights = c->unit ? nullptr : c->weights2.p;
@@ -1143,7 +1155,7 @@ int mvgpu_destroy(mvgpu_ctx *c) {
   c->scratch.release(); c->cub_tmp.release(); c->coll_tmp.release(); c->sorted_tmp.release(); c->remote_list.release(); c->remote_pos.release(); c->ghost_gid.release(); c->send_gid.release();
   c->bfs_key.release(); c->sortkey.release(); c->sortkey2.release(); c->deg_new.release(); c->rowptr2.release();
   c->ids.release(); c->perm.release(); c->inv.release(); c->lab.release(); c->tails2.release(); c->final_orig.release();
-  c->weights2.release(); c->level_flags.release();
+  c->weights2.release(); c->bfs_level_count.release();
   c->p2p.release();
   c->send_lid.release(); c->send_buf.release(); c->heavy_list.release(); c->hkeys.release(); c->hvals_i.release();
   c->hvals_d.release(); c->heavy_off.release();
