@@ -38,7 +38,12 @@ def _worker(rank, world, port, case_name, out_dir, opts):
     from minivite_b200 import dist as D
     from minivite_b200 import gpu as G
     R = D.Ranks("gloo")
-    golden = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_traces.json")))["cases"]
+    if case_name.startswith("wexact:"):          # a dyadic-weight case of weighted_exact_traces.json
+        from helpers import weighted_exact_cases
+        case_name = case_name[len("wexact:"):]
+        golden = weighted_exact_cases()
+    else:
+        golden = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_traces.json")))["cases"]
     case = dict(golden[case_name])
     case["nranks"] = world                       # re-split the same global graph over `world` GPU ranks
     if case["kind"] == "rgg":
@@ -136,6 +141,21 @@ def test_multi_gpu_weighted_and_heavy(tmp_path, golden):
     check(res, golden["rgg_n16384_p2"])
     res = run_ranks(tmp_path, 2, "rgg_n16384_p2", force_weighted=1)
     check(res, golden["rgg_n16384_p2"])
+
+
+@pytest.mark.parametrize("name,world", [("rgg_n16384_s1", 2), ("rgg_n16384_s1", 4), ("rmat_s14", 2), ("rmat_s14", 4),
+                                        ("random_n6000_d8_hubs3_hub_deg3000_multi200", 2), ("hand_self_loops_w", 2)])
+def test_multi_gpu_weighted_exact(tmp_path, name, world):
+    """Dyadic weights (tests/golden/weighted_exact_traces.json): every sum is exact, so p GPUs reproduce the 1-rank
+    reference trace bit for bit, weighted remote community reads and hub tables included."""
+    if ngpus() < world:
+        pytest.skip(f"needs {world} GPUs")
+    from helpers import weighted_exact_cases
+    case = weighted_exact_cases()[name]
+    for opts in ({}, {"reorder": 1, "region_size": 64}):
+        res = run_ranks(tmp_path, world, "wexact:" + name, **opts)
+        assert res["timings"]["unit_weight"] == 0
+        check(res, case)
 
 
 def test_cli_multi_gpu(tmp_path, golden):

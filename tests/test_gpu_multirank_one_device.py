@@ -89,6 +89,13 @@ def test_options_on_one_device(golden):
     for opts in ({"reorder": 1, "region_size": 64}, {"scan_variant": 3}, {"scan_variant": 4}, {"scan_variant": 3, "reorder": 1, "region_size": 64},
                  {"first_iter": 0}, {"force_heavy_deg": 8}, {"force_weighted": 1}, {"compact_upload": 1}):
         check(run_threads(golden, "rgg_n16384_p2", 2, **opts), golden["rgg_n16384_p2"])
+    # dyadic weights (k/4, self loops 2.5 and 0.75): every sum is exact, so the weighted path is bit-exact across ranks
+    for name in ("hand_weighted20_p1", "hand_weighted20_p2"):
+        for opts in ({}, {"scan_variant": 3}, {"force_heavy_deg": 2}):
+            res = run_threads(golden, name, 2, **opts)
+            assert res["timings"]["unit_weight"] == 0
+            check(res, golden[name])
+    # Euclidean weights are not exactly representable: the sums' last bits depend on their order, hence the tolerance
     res = run_threads(golden, "file_rgg_n16384_s2_w_p2", 2)
     assert abs(res["mod"] - float(golden["file_rgg_n16384_s2_w_p2"]["modularity"])) <= 1e-6
 

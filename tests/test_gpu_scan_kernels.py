@@ -5,20 +5,22 @@ synchronous bulk copies), vertices handed to the high-degree kernel, ragged last
 import numpy as np
 import pytest
 
-from helpers import assert_trace_matches
+from helpers import assert_trace_matches, dyadic_exponent, random_graph
 from test_gpu_parity import as_single, gpu, is_weighted, run_single  # noqa: F401  (gpu is a fixture)
 
 pytestmark = pytest.mark.gpu
-EDGE = np.dtype([("tail", "<i8"), ("weight", "<f8")])
 VARIANTS = [3, 4, 5, 6]
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
 def test_golden_cases(gpu, golden, variant):
+    """Every golden case, bit-exact where the weights are exactly representable (unit, and hand_weighted20's k/4 on 1
+    and 2 ranks); the Euclidean -w RGG weights make the last bits depend on the order of the sums, so those 1-rank cases
+    keep |dQ| <= 1e-6."""
     for name, case in golden.items():
         nv, parts, rowptr, edges = as_single(case)
         res = run_single(gpu, parts, rowptr, edges, nv, scan_variant=variant)
-        if is_weighted(name, case):
+        if is_weighted(name, case) and dyadic_exponent(edges["weight"]) is None:
             if case["nranks"] == 1:
                 assert abs(res["modularity"] - float(case["modularity"])) <= 1e-6, name
         else:
@@ -35,41 +37,6 @@ def test_options_keep_results(gpu, golden, variant):
                      {"force_heavy_deg": 8, "reorder": 1, "region_size": 32}, {"force_weighted": 1, "reorder": 1, "force_heavy_deg": 5}):
             res = run_single(gpu, parts, rowptr, edges, nv, scan_variant=variant, **opts)
             assert_trace_matches(case, res["iters"], res["modularity"], res["trace"], None, res["comm"] if "comm" in case else None)
-
-
-def random_graph(n, avg_deg, seed, hubs=0, hub_deg=0, self_loops=0, multi=0, blocks=0):
-    """Symmetric random multigraph in the reference's CSR format (unit weights), adjacency sorted by tail.
-    blocks > 0: planted partition (90 % of the edges inside `blocks` equal groups of scattered vertex ids)."""
-    rng = np.random.default_rng(seed)
-    m = n * avg_deg // 2
-    a, b = rng.integers(0, n, m), rng.integers(0, n, m)
-    if blocks:
-        inside = rng.random(m) < 0.9
-        b = np.where(inside, (b // blocks) * blocks + a % blocks, b) % n      # same residue class = same block
-    keep = a != b
-    a, b = a[keep], b[keep]
-    for h in range(hubs):
-        t = rng.choice(n, hub_deg, replace=False)
-        t = t[t != h]
-        a, b = np.concatenate([a, np.full(len(t), h)]), np.concatenate([b, t])
-    key = np.unique(np.minimum(a, b) * n + np.maximum(a, b))          # simple graph first
-    a, b = key // n, key % n
-    if multi:
-        pick = rng.integers(0, len(a), multi)
-        a, b = np.concatenate([a, a[pick]]), np.concatenate([b, b[pick]])
-    src, dst = np.concatenate([a, b]), np.concatenate([b, a])
-    if self_loops:
-        s = rng.integers(0, n, self_loops)
-        src, dst = np.concatenate([src, s]), np.concatenate([dst, s])
-    order = np.lexsort((dst, src))
-    src, dst = src[order], dst[order]
-    rowptr = np.zeros(n + 1, np.int64)
-    np.add.at(rowptr, src + 1, 1)
-    rowptr = np.cumsum(rowptr)
-    edges = np.zeros(len(dst), EDGE)
-    edges["tail"] = dst
-    edges["weight"] = 1.0
-    return rowptr, edges
 
 
 @pytest.mark.parametrize("variant", VARIANTS)

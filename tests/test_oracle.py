@@ -5,7 +5,7 @@ import os
 import numpy as np
 import pytest
 
-from helpers import assert_trace_matches, case_graph
+from helpers import assert_dyadic_exact, assert_trace_matches, case_graph, global_csr, weighted_exact_cases
 from oracle import oracle as O
 
 
@@ -121,6 +121,42 @@ def test_rgg_radius_matches_survey_table():
     assert abs(hg.rgg_radius(16384) - 1.249e-2) < 5e-6          # SURVEY.md section 8 config table (graph.hpp:629-631)
     assert abs(hg.rgg_radius(16777216) - 4.567e-4) < 5e-8
     assert abs(hg.rgg_radius(67108864, 8) - 2.341e-4) < 5e-8
+
+
+WEIGHTED_EXACT = weighted_exact_cases()
+
+
+def test_weighted_exact_goldens_cover_the_intended_paths():
+    """The dyadic-weight goldens: enough of them, exactly representable, weights that matter, and the shapes that reach
+    the weighted staging sub-ranges, the high-degree kernel unforced and the auto renumbering."""
+    assert len(WEIGHTED_EXACT) >= 20
+    for name, case in WEIGHTED_EXACT.items():
+        nv, rowptr, edges = global_csr(case)
+        assert len(edges) == case["ne"] and nv == case["nv"], name
+        assert assert_dyadic_exact(nv, rowptr, edges) == case["dyadic_j"], name
+        assert int(np.diff(rowptr).max()) == case["maxdeg"], name
+        if not case["scaled_unit"]:
+            assert (edges["weight"] != 1.0).any(), name
+    maxdeg = [c["maxdeg"] for c in WEIGHTED_EXACT.values()]
+    assert max(maxdeg) > 2048 and sum(d > 2048 for d in maxdeg) >= 2           # above every tile capacity
+    assert max(c["nv"] for c in WEIGHTED_EXACT.values()) >= 131072
+
+
+@pytest.mark.parametrize("name", sorted(WEIGHTED_EXACT))
+@pytest.mark.parametrize("shards", [1, 2, 4])
+def test_oracle_matches_weighted_exact_goldens(name, shards):
+    """Dyadic weights make every fp64 sum exact: the C restatement reproduces the unmodified reference's weighted trace
+    bit for bit -- iterations, every (modularity, moved, hash), final modularity, 1/(2m), final assignment -- on 1, 2 and
+    4 shards of the same graph."""
+    case = WEIGHTED_EXACT[name]
+    if case["nv"] < 2 * shards:
+        pytest.skip("fewer than two vertices per shard")
+    parts, rps, eds, _ = case_graph(dict(case, nranks=shards))
+    r = O.louvain(parts, rps, eds)
+    comm = np.concatenate(r["comm"])
+    assert_trace_matches(case, r["iters"], r["modularity"], r["trace"], r["chash_final"], comm)
+    assert repr(r["modularity"]) == repr(float(case["modularity"]))
+    assert repr(r["constant"]) == case["constant"], name
 
 
 def test_oracle_matches_power_law_goldens(golden_rmat):
