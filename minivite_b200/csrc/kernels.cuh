@@ -923,6 +923,7 @@ __global__ void __launch_bounds__(256) k_collect_heavy(int lnv, const uint32_t *
 // ----------------------------------------------------------------------------------------------
 constexpr unsigned int kBfsRegionBits = 22;
 constexpr unsigned int kBfsUnreached = 0xFFFFFFFFu;
+constexpr long long kBfsMaxRegions = (1LL << kBfsRegionBits) - 1;   // setup_run widens the regions to stay below this
 // edges per lane whose loads are all issued before the first compare (BFS expansion and CSR permute); on H100 at
 // config 2, 16 beat 8 and 4 in both kernels (DESIGN.md §3.3)
 constexpr int kEdgeBatch = 16;

@@ -138,6 +138,14 @@ struct mvgpu_ctx {
   bool reordered = false;
   int relabel = 0;
   double reorder_s = 0.0;
+  // what the last setup decided, kept on the host for mv_layout_readback (a test hook, not in mvgpu.h); every value is
+  // one that setup_run or run_louvain already had on the host
+  int lay_want = 0, lay_stride = 0;
+  long long lay_nregions = 0;
+  long long lay_span[2] = {-1, -1};   // k_span_sample's sum and count; -1: the sample did not run
+  int lay_unordered = 0, lay_has_self = 0;
+  bool lay_first_ran = false;         // iteration 1 launched k_scan_pw's FIRST instantiation
+  const int32_t *lay_tails = nullptr; // the compact tails before renumbering (c->tails or the uploaded compact array)
   DevBuf<double> self_d, vdeg;
   // state
   DevBuf<int32_t> comm_a, comm_b;
@@ -429,8 +437,10 @@ int launch_scan_t(mvgpu_ctx *c, const ScanParams &sp, bool first) {
     }
     const int ngroups = (int)((c->lnv + 31) / 32);
     const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, pw_ctas_per_sm * c->num_sms);
-    if (UNIT && first) k_scan_pw<UNIT, MULTI, TRACE, UNIT><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
-    else k_scan_pw<UNIT, MULTI, TRACE, false><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
+    if (UNIT && first) {
+      k_scan_pw<UNIT, MULTI, TRACE, UNIT><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
+      c->lay_first_ran = true;
+    } else k_scan_pw<UNIT, MULTI, TRACE, false><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
     c->tm.kernel_launches++; c->tm.scan_launches++;
   } else if (tiles > 0) {
     k_scan_ws<UNIT, MULTI, TRACE><<<tiles, kTileV, UNIT ? sizeof(int32_t) * kECap : smem, c->stream>>>(sp);
@@ -623,6 +633,10 @@ int setup_run(mvgpu_ctx *c) {
   // ---- locality renumbering (see kernels.cuh): decide, then BFS regions -> sort -> permute the compact CSR
   c->reordered = false;
   c->relabel = 0;
+  c->lay_tails = src_tails;
+  c->lay_span[0] = c->lay_span[1] = -1;
+  c->lay_nregions = 0;
+  c->lay_first_ran = false;
   {
     int want = c->opt_reorder == 1 ? 1 : 0;
     if (c->opt_reorder == 2 && lnv >= 65536) {
@@ -633,7 +647,13 @@ int setup_run(mvgpu_ctx *c) {
       CK(cudaMemcpyAsync(sp2, &d_sc->span_sum, sizeof sp2, cudaMemcpyDeviceToHost, s));
       CK(cudaStreamSynchronize(s));
       if (sp2[1] > 0 && (double)sp2[0] / (double)sp2[1] > (double)lnv / 64.0) want = 1;
+      c->lay_span[0] = (long long)sp2[0]; c->lay_span[1] = (long long)sp2[1];
     }
+    // region ids have kBfsRegionBits bits: past 2^22 - 1 regions they would spill into the level field (and region
+    // 2^22 - 1 at level 1023 would read as kBfsUnreached), so very large shards get proportionally larger regions
+    const int stride = (int)std::max<long long>(c->opt_region, (lnv + kBfsMaxRegions - 1) / kBfsMaxRegions);
+    c->lay_want = want;
+    c->lay_stride = stride;
     int any = want;
     if (c->nranks > 1) {
       long long hv = want;
@@ -654,15 +674,16 @@ int setup_run(mvgpu_ctx *c) {
         int occ = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_msbfs, 256, 0));
         if (occ < 1) return fail("k_msbfs cannot be made resident");
-        int ilnv = (int)lnv, stride = c->opt_region, ml = max_levels;
+        int ilnv = (int)lnv, st = stride, ml = max_levels;
         const uint32_t *rp = src_rowptr; const int32_t *tl = src_tails; uint32_t *key = c->bfs_key.p;
         // the BFS queue and its level bitmaps (4 bits per vertex) live in ids and sortkey2, which k_bfs_sortkeys and the
         // sort only write after the BFS
         int32_t *q = c->ids.p; unsigned int *lc = c->bfs_level_count.p; uint32_t *lm = c->sortkey2.p;
-        void *args[] = {&ilnv, &rp, &tl, &key, &stride, &ml, &q, &lc, &lm};
+        void *args[] = {&ilnv, &rp, &tl, &key, &st, &ml, &q, &lc, &lm};
         CK(cudaLaunchCooperativeKernel((void *)k_msbfs, dim3(occ * nsm), dim3(256), args, 0, s));
         // sort by (region, level): only the bits that can be set take part (one radix pass less than a 32-bit sort)
         const long long nregions = (lnv + stride - 1) / stride;
+        c->lay_nregions = nregions;
         int sort_bits = (int)kBfsLevelBits;
         while ((1LL << (sort_bits - (int)kBfsLevelBits)) <= nregions && sort_bits < 32) sort_bits++;
         const unsigned int unreached_key = sort_bits >= 32 ? 0xFFFFFFFFu : ((1u << sort_bits) - 1u);
@@ -761,6 +782,8 @@ int setup_run(mvgpu_ctx *c) {
   if (c->f32) c->constant = (double)(float)(1.0 / (double)(float)h.total_weight);   // dspl.hpp:129 with GraphWeight = float
   const int has_self = h.has_self ? 1 : 0;
   c->simple_sorted = c->unit && !h.unordered && !has_self;
+  c->lay_unordered = h.unordered ? 1 : 0;
+  c->lay_has_self = has_self;
   if (c->maxdeg > heavy_deg) {
     c->nheavy = h.heavy_count;
     std::vector<int32_t> hl(c->nheavy);
@@ -1597,6 +1620,43 @@ int mvgpu_get_constant(mvgpu_ctx *c, double *out) {
 int mvgpu_get_shard_info(mvgpu_ctx *c, int64_t *info6) {
   if (!c || !info6) return fail("null argument");
   info6[0] = c->lnv; info6[1] = c->lne; info6[2] = c->nghost; info6[3] = c->nsend; info6[4] = c->nheavy; info6[5] = c->maxdeg;
+  return 0;
+}
+
+// Test hook, deliberately not declared in mvgpu.h: what the last mvgpu_louvain decided about the layout and which
+// layout it built, valid until the next run.  info16 (may be NULL): want, relabel, reordered, region stride, regions,
+// span sum, span count (-1, -1 when the sample did not run), unordered, has_self, simple_sorted, FIRST launched, unit,
+// nlow, nghost, lnv, lne.  Arrays (each may be NULL): the compact CSR before renumbering (rowptr lnv+1, tails lne, in
+// slot numbering), bfs_key (lnv, this rank renumbered), perm / inv / lab (lnv, some rank renumbered), the renumbered
+// CSR (rowptr2 lnv+1, tails2 lne, weights2 lne on the weighted path).  Asking for an array the run did not build fails.
+int mv_layout_readback(mvgpu_ctx *c, int64_t *info16, uint32_t *rowptr, int32_t *tails, uint32_t *bfs_key, int32_t *perm,
+                       int32_t *inv, int32_t *lab, uint32_t *rowptr2, int32_t *tails2, double *weights2) {
+  if (!c) return fail("null ctx");
+  if (!c->d_final) return fail("no run yet");
+  if (info16) {
+    const int64_t v[16] = {c->lay_want, c->relabel, c->reordered ? 1 : 0, c->lay_stride, c->lay_nregions, c->lay_span[0],
+                           c->lay_span[1], c->lay_unordered, c->lay_has_self, c->simple_sorted ? 1 : 0,
+                           c->lay_first_ran ? 1 : 0, c->unit ? 1 : 0, c->roff.empty() ? 0 : c->roff[c->rank], c->nghost,
+                           c->lnv, c->lne};
+    memcpy(info16, v, sizeof v);
+  }
+  const bool has_bfs = c->lay_want && c->relabel && c->lnv > 0, has_perm = c->relabel && c->lnv > 0;
+  if ((bfs_key && !has_bfs) || ((perm || inv || lab) && !has_perm) || ((rowptr2 || tails2) && !c->reordered) ||
+      (weights2 && (!c->reordered || c->unit)))
+    return fail("mv_layout_readback: the last run did not build that array");
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  const size_t nv = (size_t)c->lnv, ne = (size_t)c->lne;
+  if (rowptr) CK(cudaMemcpyAsync(rowptr, c->rowptr.p, sizeof(uint32_t) * (nv + 1), cudaMemcpyDeviceToHost, s));
+  if (tails && ne) CK(cudaMemcpyAsync(tails, c->lay_tails, sizeof(int32_t) * ne, cudaMemcpyDeviceToHost, s));
+  if (bfs_key) CK(cudaMemcpyAsync(bfs_key, c->bfs_key.p, sizeof(uint32_t) * nv, cudaMemcpyDeviceToHost, s));
+  if (perm) CK(cudaMemcpyAsync(perm, c->perm.p, sizeof(int32_t) * nv, cudaMemcpyDeviceToHost, s));
+  if (inv) CK(cudaMemcpyAsync(inv, c->inv.p, sizeof(int32_t) * nv, cudaMemcpyDeviceToHost, s));
+  if (lab) CK(cudaMemcpyAsync(lab, c->lab.p, sizeof(int32_t) * nv, cudaMemcpyDeviceToHost, s));
+  if (rowptr2) CK(cudaMemcpyAsync(rowptr2, c->rowptr2.p, sizeof(uint32_t) * (nv + 1), cudaMemcpyDeviceToHost, s));
+  if (tails2 && ne) CK(cudaMemcpyAsync(tails2, c->tails2.p, sizeof(int32_t) * ne, cudaMemcpyDeviceToHost, s));
+  if (weights2 && ne) CK(cudaMemcpyAsync(weights2, c->weights2.p, sizeof(double) * ne, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
   return 0;
 }
 

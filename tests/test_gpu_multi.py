@@ -38,19 +38,25 @@ def _worker(rank, world, port, case_name, out_dir, opts):
     from minivite_b200 import dist as D
     from minivite_b200 import gpu as G
     R = D.Ranks("gloo")
-    if case_name.startswith("wexact:"):          # a dyadic-weight case of weighted_exact_traces.json
-        from helpers import weighted_exact_cases
-        case_name = case_name[len("wexact:"):]
-        golden = weighted_exact_cases()
+    if case_name == "keep_order":                # even ranks keep their numbering, odd ranks renumber (test_gpu_layout.py)
+        from helpers import split_global
+        from test_gpu_layout import keep_order_graph
+        nv, parts, rowptr, edges = keep_order_graph(world)
+        _, rps, eds = split_global(nv, rowptr, edges, world)
     else:
-        golden = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_traces.json")))["cases"]
-    case = dict(golden[case_name])
-    case["nranks"] = world                       # re-split the same global graph over `world` GPU ranks
-    if case["kind"] == "rgg":
-        case = dict(case, kind="file_rgg", strips=golden[case_name]["nranks"], unit_weight="-w" not in case["args"])
-        if "-l" in golden[case_name]["args"]:
-            raise RuntimeError("lcg cases are not re-split here")
-    parts, rps, eds, keep = case_graph(case)
+        if case_name.startswith("wexact:"):      # a dyadic-weight case of weighted_exact_traces.json
+            from helpers import weighted_exact_cases
+            case_name = case_name[len("wexact:"):]
+            golden = weighted_exact_cases()
+        else:
+            golden = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_traces.json")))["cases"]
+        case = dict(golden[case_name])
+        case["nranks"] = world                   # re-split the same global graph over `world` GPU ranks
+        if case["kind"] == "rgg":
+            case = dict(case, kind="file_rgg", strips=golden[case_name]["nranks"], unit_weight="-w" not in case["args"])
+            if "-l" in golden[case_name]["args"]:
+                raise RuntimeError("lcg cases are not re-split here")
+        parts, rps, eds, keep = case_graph(case)
     ident = R.broadcast_bytes(G.get_unique_id() if rank == 0 else None, G.UNIQUE_ID_BYTES)
     g = G.LouvainGPU(rank, rank, world)
     g.comm_init(ident)
@@ -63,9 +69,11 @@ def _worker(rank, world, port, case_name, out_dir, opts):
     tr = g.trace()
     info = g.shard_info()
     allc = R.gather_arrays(comm)
+    decided = R.gather_arrays(np.array([g.timings()["reordered"]], np.int64))
     if rank == 0:
         json.dump({"mod": repr(mod), "iters": iters, "trace": [[repr(float(t["modularity"])), int(t["moved"]), int(t["chash"])] for t in tr],
-                   "comm": [int(x) for x in np.concatenate(allc)], "info": info, "timings": g.timings()},
+                   "comm": [int(x) for x in np.concatenate(allc)], "info": info, "timings": g.timings(),
+                   "reordered": [int(x) for x in np.concatenate(decided)]},
                   open(os.path.join(out_dir, "res.json"), "w"))
     g.close()
     R.shutdown()
@@ -116,6 +124,26 @@ def test_multi_gpu_with_renumbering(tmp_path, golden):
         check(res, golden[name])
     res = run_ranks(tmp_path, 2, "rgg_n16384_p2", reorder=1, region_size=64, scan_variant=3)
     check(res, golden["rgg_n16384_p2"])
+
+
+@pytest.mark.parametrize("world", [2, 4])
+def test_multi_gpu_rank_that_keeps_its_numbering(tmp_path, world):
+    """Auto mode with mixed decisions (tests/test_gpu_layout.py keep_order_graph): the even ranks keep their numbering
+    while the odd ones renumber; bit-exact against the C oracle on the same shards."""
+    if ngpus() < world:
+        pytest.skip(f"needs {world} GPUs")
+    from helpers import split_global
+    from oracle import oracle as O
+    from test_gpu_layout import keep_order_graph
+    res = run_ranks(tmp_path, world, "keep_order")
+    assert res["reordered"] == [r % 2 for r in range(world)]
+    nv, parts, rowptr, edges = keep_order_graph(world)
+    _, rps, eds = split_global(nv, rowptr, edges, world)
+    ref = O.louvain(parts, rps, eds)
+    assert res["iters"] == ref["iters"] and float(res["mod"]) == ref["modularity"]
+    assert [[float(m), mv, h] for m, mv, h in res["trace"]] == \
+        [[float(t["modularity"]), int(t["moved"]), int(t["chash"])] for t in ref["trace"]]
+    assert res["comm"] == [int(x) for x in np.concatenate(ref["comm"])]
 
 
 def test_multi_gpu_nccl_collectives_mode(tmp_path, golden):
