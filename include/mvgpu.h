@@ -102,6 +102,18 @@ int mvgpu_download_shard(mvgpu_ctx *ctx, int64_t *edge_indices, void *edge_list)
  * (dspl.hpp:1430); *modularity is prevMod (dspl.hpp:1440).  Collective over all ranks. */
 int mvgpu_louvain(mvgpu_ctx *ctx, double lower, double thresh, int *iters, double *modularity);
 
+/* Warm start: the next runs on this shard start from `comm` (lnv global community ids in the caller's vertex numbering,
+ * the form mvgpu_get_communities returns) instead of singletons.  Every id must lie in [0, nv); id c names the vertex
+ * whose owner keeps the community's Comm record, as in the reference -- the community need not contain vertex c, need
+ * not be contiguous and may be owned by another rank.  The array is copied and validated at call time (errors are
+ * local: no collective).  It stays in effect for every later mvgpu_louvain on this shard until NULL clears it or the next
+ * upload / attach / generate replaces the shard.  In a multi-rank run every rank or none must set one (checked at the
+ * start of mvgpu_louvain, which then fails on every rank).  Resuming a run stopped by the "stop_after" option from its
+ * assignment with lower = its returned modularity continues it exactly (DESIGN.md §3.9).  Not for mvgpu_louvain32. */
+int mvgpu_set_initial_communities(mvgpu_ctx *ctx, const int64_t *comm);
+/* 1 if the last mvgpu_louvain ended on the reference's exit test, 0 if "stop_after" ended it first. */
+int mvgpu_get_converged(mvgpu_ctx *ctx, int *converged);
+
 /* currComm of this rank's vertices at exit (global community ids), lnv entries. */
 int mvgpu_get_communities(mvgpu_ctx *ctx, int64_t *out);
 /* Same values left in device memory (int32 global ids); valid until the next mvgpu_louvain. */
@@ -125,7 +137,10 @@ int mvgpu_get_communities_device(mvgpu_ctx *ctx, const int32_t **d_out);
  * required when several ranks share one device, which NCCL refuses; needs comm_mode 1; default 0), "compact_upload" (1:
  * mvgpu_upload_shard sends unit-weight shards as 4-byte tails narrowed on the host; 2: the copy engine additionally
  * takes raw chunks from the far end of the array whenever no narrowed chunk is ready (narrowed on the device);
- * 0 (default) = the 16-byte records as they are), "host_threads" (threads of that host pass, default 8).
+ * 0 (default) = the 16-byte records as they are), "host_threads" (threads of that host pass, default 8), "stop_after"
+ * (0 = off (default); k > 0: end the run successfully after k ACCEPTED iterations: *iters = k, *modularity = prevMod
+ * after iteration k -- the `lower` to resume with --, k trace records, mvgpu_get_communities returns the assignment
+ * after iteration k; if the exit test fires first the run ends as without it, see mvgpu_get_converged).
  * The environment variable MVGPU_OPTIONS="name=value,name=value" presets options for every context of the process. */
 /* In a multi-rank run every rank must set the same options (they change which collectives a run issues). */
 int mvgpu_set_option(mvgpu_ctx *ctx, const char *name, int64_t value);
@@ -151,6 +166,7 @@ int mvgpu_get_shard_info(mvgpu_ctx *ctx, int64_t *info6);
  * and the comparison is by tolerance.  parts / edge_indices are int32 here, like every GraphElem of that build. */
 int mvgpu_upload_shard32(mvgpu_ctx *ctx, int32_t nv_global, const int32_t *parts, int32_t lnv, int32_t lne,
                          const int32_t *edge_indices, const void *edge_list8);
+/* Fails while an initial assignment or "stop_after" is set (warm start is a 64-bit surface feature). */
 int mvgpu_louvain32(mvgpu_ctx *ctx, float lower, float thresh, int *iters, float *modularity);
 int mvgpu_get_communities32(mvgpu_ctx *ctx, int32_t *out);
 

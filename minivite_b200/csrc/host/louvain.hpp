@@ -22,6 +22,9 @@ struct GpuRankContext {
   std::vector<GraphElem> *comm_out = nullptr;     // final currComm of this rank (the reference drops it, dspl.hpp:1432-1438)
   mvgpu_timings timings{};
   std::vector<mvgpu_iter_trace> iter_trace;
+  const std::vector<GraphElem> *init_comm = nullptr;   // -i: starting assignment of this rank's vertices (global ids)
+  int stop_after = 0;                                  // -k: stop after that many accepted iterations (0 = off)
+  bool stopped = false;                                // the run ended by stop_after, not by the exit test
 };
 
 [[noreturn]] inline void mv_abort(const std::string &where) {
@@ -55,6 +58,17 @@ inline int mv_env_repeat() {
   return n < 1 ? 1 : n;
 }
 
+// -i / -k: hand the starting assignment and the stop point to the library (after the shard exists)
+inline void mv_apply_warm_start(mvgpu_ctx *ctx, const GpuRankContext &rc) {
+  if (rc.init_comm && mvgpu_set_initial_communities(ctx, rc.init_comm->data())) mv_abort("mvgpu_set_initial_communities");
+  if (rc.stop_after && mvgpu_set_option(ctx, "stop_after", rc.stop_after)) mv_abort("stop_after");
+}
+inline void mv_read_converged(mvgpu_ctx *ctx, GpuRankContext &rc) {
+  int conv = 1;
+  if (mvgpu_get_converged(ctx, &conv)) mv_abort("mvgpu_get_converged");
+  rc.stopped = conv == 0;
+}
+
 // MVGPU_SCAN_TIMES=1: print the duration of every scan launch of the last phase (ms) on stderr
 inline void mv_print_scan_times(mvgpu_ctx *ctx, int me) {
   if (me != 0 || !std::getenv("MVGPU_SCAN_TIMES")) return;
@@ -85,10 +99,12 @@ inline GraphWeight distLouvainMethod(const int me, const int nprocs, const Graph
   if (mvgpu_upload_shard(ctx, dg.get_nv(), dg.parts().data(), dg.get_lnv(), dg.get_lne(), dg.edge_indices_.data(),
                          dg.edge_list_.data()))
     mv_abort("mvgpu_upload_shard");
+  mv_apply_warm_start(ctx, rc);
   double mod = 0.0;
   for (int rep = mv_env_repeat(); rep > 0; rep--)
     if (mvgpu_louvain(ctx, lower, thresh, &iters, &mod)) mv_abort("mvgpu_louvain");
   mvgpu_get_timings(ctx, &rc.timings);
+  mv_read_converged(ctx, rc);
   mv_print_scan_times(ctx, me);
   if (rc.trace) {
     int n = 0;
@@ -121,11 +137,13 @@ inline GraphWeight distLouvainMethodOnDeviceRGG(const int me, const int nprocs, 
   if (mvgpu_generate_rgg_shard_ex(ctx, nv, unitEdgeWeight ? 1 : 0, lcg ? 1 : 0, randomEdgePercent, &lne64)) mv_abort("mvgpu_generate_rgg_shard");
   gen_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   lne = lne64;
+  mv_apply_warm_start(ctx, rc);
   before_louvain();
   double mod = 0.0;
   for (int rep = mv_env_repeat(); rep > 0; rep--)
     if (mvgpu_louvain(ctx, lower, thresh, &iters, &mod)) mv_abort("mvgpu_louvain");
   mvgpu_get_timings(ctx, &rc.timings);
+  mv_read_converged(ctx, rc);
   mv_print_scan_times(ctx, me);
   if (rc.trace) {
     int n = 0;

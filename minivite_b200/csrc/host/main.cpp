@@ -8,6 +8,8 @@
 //   -l         LCG random numbers         -p <pct> extra random edges      -s  print the graph
 // additions: -g <gpus> (default 1)   -o <prefix> dump final communities per rank   -T per-iteration trace on stderr
 //            -D generate the RGG on the GPU (same graph; with -n, also -w, -l and -p; without -s)
+//            -i <prefix> start from the communities an earlier -o <prefix> wrote   -k <n> stop after n accepted
+//            iterations (prints STOPPED iters=<n> prevMod=<v>)   -L <v> starting `lower` (default -1; resume: -L <v>)
 #include <getopt.h>
 #include <sys/mman.h>
 #include <sys/wait.h>
@@ -27,7 +29,9 @@
 #include "louvain.hpp"
 #include "rgg.hpp"
 
-static std::string inputFileName, dumpPrefix;
+static std::string inputFileName, dumpPrefix, initPrefix;
+static int stopAfter = 0;
+static GraphWeight lowerStart = -1.0;
 static int me = 0, nprocs = 1;
 static int ranksPerNode = 1;
 static GraphElem nvRGG = 0;
@@ -80,7 +84,7 @@ static long long reduce_sum_ll(long long v) {
 
 static void parseCommandLine(const int argc, char *const argv[]) {
   int ret;
-  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TD")) != -1) {
+  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:")) != -1) {
     switch (ret) {
       case 'f': inputFileName.assign(optarg); break;
       case 'b': readBalanced = true; break;
@@ -95,6 +99,9 @@ static void parseCommandLine(const int argc, char *const argv[]) {
       case 'o': dumpPrefix.assign(optarg); break;
       case 'T': traceIters = true; break;
       case 'D': deviceGenerate = true; break;
+      case 'i': initPrefix.assign(optarg); break;
+      case 'k': stopAfter = atoi(optarg); break;
+      case 'L': lowerStart = atof(optarg); break;
       default: assert(0 && "Option not recognized!!!"); break;
     }
   }
@@ -118,6 +125,7 @@ static void parseCommandLine(const int argc, char *const argv[]) {
   if (deviceGenerate && (!generateGraph || showGraph)) {
     std::cerr << "-D (generate the RGG on the GPU) needs -n and excludes -s." << std::endl; exit(99);
   }
+  if (stopAfter < 0) { std::cerr << "-k needs a number of iterations >= 0." << std::endl; exit(99); }
 }
 
 int main(int argc, char *argv[]) {
@@ -220,7 +228,29 @@ int main(int argc, char *argv[]) {
     memcpy(rc.unique_id, shm->unique_id, sizeof rc.unique_id);
   }
 
-  GraphWeight currMod = -1.0;
+  // -i: this rank's slice of an earlier run's -o dump ({base, lnv} header, then lnv global community ids)
+  std::vector<GraphElem> initComm;
+  if (!initPrefix.empty()) {
+    const long long want_base = deviceGenerate ? (long long)(nvRGG / nprocs) * me : (long long)g->get_base(me);
+    const long long want_lnv = deviceGenerate ? (long long)(nvRGG / nprocs) : (long long)g->get_lnv();
+    const std::string fn = initPrefix + "." + std::to_string(me);
+    FILE *f = fopen(fn.c_str(), "rb");
+    long long hdr[2] = {-1, -1};
+    bool ok = f && fread(hdr, 8, 2, f) == 2 && hdr[0] == want_base && hdr[1] == want_lnv;
+    if (ok) {
+      initComm.resize((size_t)want_lnv);
+      ok = fread(initComm.data(), sizeof(GraphElem), initComm.size(), f) == initComm.size();
+    }
+    if (f) fclose(f);
+    if (!ok)
+      fprintf(stderr, "[miniVite_b200] -i %s: cannot read %s or its header {base %lld, lnv %lld} does not match this rank's "
+              "shard {base %lld, lnv %lld}\n", initPrefix.c_str(), fn.c_str(), hdr[0], hdr[1], want_base, want_lnv);
+    if (reduce_sum_ll(ok ? 0 : 1)) abort_all(99);       // every rank leaves, not only the one with the bad file
+    rc.init_comm = &initComm;
+  }
+  rc.stop_after = stopAfter;
+
+  GraphWeight currMod = lowerStart;
   std::vector<GraphElem> ssizes, rsizes, svdata, rvdata;
   size_t ssz = 0, rsz = 0;
   int iters = 0;
@@ -286,6 +316,7 @@ int main(int argc, char *argv[]) {
             rc.timings.fold_s * 1e3, rc.timings.exchange_s * 1e3, (int)rc.timings.kernel_launches, (int)rc.timings.reordered);
     fprintf(stderr, "RESULT mod=%.17g iters=%d time=%.9g nv=%ld ne=%ld nprocs=%d threads=0\n", currMod, iters, avgd,
             (long)nv_rep, (long)ne_rep, nprocs);
+    if (rc.stopped) fprintf(stderr, "STOPPED iters=%d prevMod=%.17g\n", iters, currMod);
   }
   rank_barrier();
   delete g;   // nullptr with -D

@@ -1268,4 +1268,66 @@ __global__ void __launch_bounds__(256) k_apply_inv(int32_t *lid, int n, const in
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) lid[i] = inv[lid[i]];
 }
 
+// ----------------------------------------------------------------------------------------------
+// Warm start (mvgpu_set_initial_communities): a given assignment replaces the singleton init of k_vertex_init.  The
+// reference loop carries only currComm, the Comm aggregates of currComm and prevMod from one iteration to the next,
+// so rebuilding the first two from the assignment continues a stopped run exactly (DESIGN.md §3.9).
+// ----------------------------------------------------------------------------------------------
+struct WarmInv {                                    // every rank's inv (old -> new local index); all nullptr when no rank renumbered
+  const int32_t *inv[kMaxRanks];
+};
+
+// cur[slot of caller-local vertex i] = internal id of community init[i]: the owner's internal id of its local vertex
+// init[i] - parts[owner], read through the owner's inv (a peer mapping for other ranks)
+__global__ void __launch_bounds__(256) k_warm_map(int lnv, const int32_t *init, const int32_t *my_inv, PeerTable pt, WarmInv m,
+                                                  int32_t *cur) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < lnv; i += gridDim.x * blockDim.x) {
+    const int c = init[i];
+    int o; long long idx;
+    locate_remote(pt, c, o, idx);
+    cur[my_inv ? my_inv[i] : i] = m.inv[o] ? (int)(pt.parts[o] + m.inv[o][idx]) : c;
+  }
+}
+
+// Comm records of the assignment, pushed as deltas into the owner's update arrays (the scan's primitive for remote
+// moves): unit path one packed (size 1, degree) 64-bit atomic per vertex, weighted path fp64 atomics
+__global__ void __launch_bounds__(256) k_warm_comm_unit(int lnv, const int32_t *cur, const uint32_t *rowptr, PeerTable pt) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) {
+    int o; long long idx;
+    locate_remote(pt, cur[v], o, idx);
+    atomicAdd(pt.upd[o] + idx, pack_delta(1, (long long)(rowptr[v + 1] - rowptr[v])));
+  }
+}
+__global__ void __launch_bounds__(256) k_warm_comm_w(int lnv, const int32_t *cur, const double *vdeg, PeerTable pt) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) {
+    int o; long long idx;
+    locate_remote(pt, cur[v], o, idx);
+    atomicAdd((unsigned long long *)(pt.usize[o] + idx), 1ULL);
+    atomicAdd(pt.udeg[o] + idx, vdeg[v]);
+  }
+}
+
+// Records from zero: cdeg / csize (or cinfo_w) := the summed deltas, the update arrays cleared for iteration 1, and
+// record 0's sum(degree^2), where k_fold_unit's incremental sum starts (acc0->la2_u must be zero on entry)
+__global__ void __launch_bounds__(256) k_warm_fold_unit(int lnv, uint32_t *cdeg, int32_t *csize, unsigned long long *upd, Acc *acc0) {
+  unsigned long long a2u = 0;
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) {
+    const unsigned long long u = upd[v];
+    const uint32_t dg = (uint32_t)u;                // both halves are non-negative sums here
+    cdeg[v] = dg;
+    csize[v] = (int32_t)(u >> 32);
+    upd[v] = 0;
+    a2u += (unsigned long long)dg * dg;
+  }
+  a2u = warp_sum(a2u);
+  if ((threadIdx.x & 31) == 0 && a2u) atomicAdd(&acc0->la2_u, a2u);
+}
+__global__ void __launch_bounds__(256) k_warm_fold_w(int lnv, CommW *cinfo_w, long long *usize, double *udeg) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) {
+    CommW c; c.size = usize[v]; c.degree = udeg[v];
+    cinfo_w[v] = c;
+    usize[v] = 0; udeg[v] = 0.0;
+  }
+}
+
 }  // namespace mv

@@ -84,9 +84,11 @@ struct DevBuf {              // grow-only device buffer (allocations are cached 
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
+constexpr int kPeerArrays = 11;
+
 struct PeerBlob {            // what every rank publishes about its community arrays
-  cudaIpcMemHandle_t h[10];
-  unsigned long long raw[10];
+  cudaIpcMemHandle_t h[kPeerArrays];
+  unsigned long long raw[kPeerArrays];
   int pid, device, unit, pad;
 };
 
@@ -184,12 +186,18 @@ struct mvgpu_ctx {
   std::vector<void *> ipc_opened;
   bool peers_ready = false, ipc_valid = false;
   int peers_unit = -1;
-  void *last_ptrs[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  unsigned last_gens[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const int32_t *peer_inv[kMaxRanks];  // every rank's inv (old -> new local index) while some rank renumbers: warm-start init only
+  void *last_ptrs[kPeerArrays] = {};
+  unsigned last_gens[kPeerArrays] = {};
   // options
   int opt_trace = 0, opt_force_weighted = 0, opt_scan_variant = 6, opt_cache_policy = 5, opt_reorder = 2, opt_region = 512, opt_comm_mode = 1, opt_compact_upload = 0, opt_host_threads = 8, opt_first_iter = 1, opt_host_transport = 0;
   long long opt_upload_chunk = 4LL << 20;
-  long long opt_max_iters = 10000, opt_force_heavy_deg = 0;
+  long long opt_max_iters = 10000, opt_force_heavy_deg = 0, opt_stop_after = 0;
+  // warm start (mvgpu_set_initial_communities): caller-numbered community ids of this shard, until the next graph
+  DevBuf<int32_t> init_comm;
+  bool have_init = false;
+  bool warm_run = false;               // the current / last run started from init_comm
+  int converged = 1;                   // the last run ended on the exit test (0: stopped by stop_after)
   // results
   bool unit = true;
   bool f32 = false;                    // shard came through mvgpu_upload_shard32: float-build arithmetic (see mvgpu.h)
@@ -307,6 +315,7 @@ int coll_barrier(mvgpu_ctx *c) {
 
 int set_graph(mvgpu_ctx *c, long long nv_global, const int64_t *parts, long long lnv, long long lne) {
   if (c->nranks > kMaxRanks) return fail("too many ranks");
+  c->have_init = false;                     // an initial assignment belongs to the shard it was given for
   if (nv_global < 0 || lnv < 0 || lne < 0) return fail("negative graph size");
   if (nv_global >= (1LL << 31)) return fail("nv_global >= 2^31: 32-bit community ids would overflow (not supported)");
   if (lne >= (1LL << 32)) return fail("lne >= 2^32 per shard: 32-bit edge offsets would overflow (not supported)");
@@ -330,18 +339,19 @@ int setup_peers(mvgpu_ctx *c, int unit) {
   if (c->nranks == 1) {
     pt.lab[0] = c->relabel ? c->lab.p : nullptr;
     pt.cdeg[0] = c->cdeg.p; pt.csize[0] = c->csize.p; pt.upd[0] = c->upd.p; pt.cinfo_w[0] = c->cinfo_w.p; pt.usize[0] = c->usize.p; pt.udeg[0] = c->udeg.p;
+    c->peer_inv[0] = c->relabel ? c->inv.p : nullptr;
     return 0;
   }
-  void *ptrs[10] = {unit ? (void *)c->cdeg.p : nullptr, unit ? (void *)c->csize.p : nullptr, unit ? (void *)c->upd.p : nullptr,
+  void *ptrs[kPeerArrays] = {unit ? (void *)c->cdeg.p : nullptr, unit ? (void *)c->csize.p : nullptr, unit ? (void *)c->upd.p : nullptr,
                     unit ? nullptr : (void *)c->cinfo_w.p, unit ? nullptr : (void *)c->usize.p,
                     unit ? nullptr : (void *)c->udeg.p, c->relabel ? (void *)c->lab.p : nullptr,
-                    (void *)c->comm_a.p, (void *)c->comm_b.p, (void *)c->p2p.p};
+                    (void *)c->comm_a.p, (void *)c->comm_b.p, (void *)c->p2p.p, c->relabel ? (void *)c->inv.p : nullptr};
   if (c->peers_ready) return 0;            // same graph, same buffers: tables are still valid
   // IPC handles are expensive to (re)open: skip the exchange when no rank's buffers moved since the last one
-  const unsigned gens[10] = {c->cdeg.gen, c->csize.gen, c->upd.gen, c->cinfo_w.gen, c->usize.gen, c->udeg.gen, c->lab.gen,
-                             c->comm_a.gen, c->comm_b.gen, c->p2p.gen};
+  const unsigned gens[kPeerArrays] = {c->cdeg.gen, c->csize.gen, c->upd.gen, c->cinfo_w.gen, c->usize.gen, c->udeg.gen, c->lab.gen,
+                                      c->comm_a.gen, c->comm_b.gen, c->p2p.gen, c->inv.gen};
   long long changed = c->ipc_valid ? 0 : 1;
-  for (int k = 0; k < 10; k++) if (ptrs[k] != c->last_ptrs[k] || (ptrs[k] && gens[k] != c->last_gens[k])) changed = 1;
+  for (int k = 0; k < kPeerArrays; k++) if (ptrs[k] != c->last_ptrs[k] || (ptrs[k] && gens[k] != c->last_gens[k])) changed = 1;
   TRY(coll_allreduce_i64(c, &changed, 1, true));
   if (changed) {
   for (void *p : c->ipc_opened) cudaIpcCloseMemHandle(p);
@@ -349,7 +359,7 @@ int setup_peers(mvgpu_ctx *c, int unit) {
   c->ipc_valid = false;
   PeerBlob mine;
   memset(&mine, 0, sizeof mine);
-  for (int k = 0; k < 10; k++) {
+  for (int k = 0; k < kPeerArrays; k++) {
     mine.raw[k] = (unsigned long long)ptrs[k];
     if (ptrs[k]) CK(cudaIpcGetMemHandle(&mine.h[k], ptrs[k]));
   }
@@ -357,9 +367,9 @@ int setup_peers(mvgpu_ctx *c, int unit) {
   std::vector<PeerBlob> all(c->nranks);
   TRY(coll_allgather(c, &mine, all.data(), sizeof(PeerBlob)));
   for (int r = 0; r < c->nranks; r++) {
-    void *q[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    void *q[kPeerArrays] = {};
     if (all[r].unit != unit) return fail("ranks disagree on the unit-weight path");
-    if (r == c->rank) { for (int k = 0; k < 10; k++) q[k] = ptrs[k]; }
+    if (r == c->rank) { for (int k = 0; k < kPeerArrays; k++) q[k] = ptrs[k]; }
     else if (all[r].pid == mine.pid) {           // same process (threads): plain UVA pointers + peer access
       if (all[r].device != c->device) {          // ranks sharing one device need no peer mapping at all
         int can = 0;
@@ -369,9 +379,9 @@ int setup_peers(mvgpu_ctx *c, int unit) {
         if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CK(e);
         cudaGetLastError();
       }
-      for (int k = 0; k < 10; k++) q[k] = (void *)all[r].raw[k];
+      for (int k = 0; k < kPeerArrays; k++) q[k] = (void *)all[r].raw[k];
     } else {
-      for (int k = 0; k < 10; k++)
+      for (int k = 0; k < kPeerArrays; k++)
         if (all[r].raw[k]) {
           CK(cudaIpcOpenMemHandle(&q[k], all[r].h[k], cudaIpcMemLazyEnablePeerAccess));
           c->ipc_opened.push_back(q[k]);
@@ -382,8 +392,9 @@ int setup_peers(mvgpu_ctx *c, int unit) {
     pt.lab[r] = (const int32_t *)q[6];
     c->peer_comm[0][r] = (int32_t *)q[7]; c->peer_comm[1][r] = (int32_t *)q[8];
     c->pp.st[r] = (P2PState *)q[9];
+    c->peer_inv[r] = (const int32_t *)q[10];
   }
-  for (int k = 0; k < 10; k++) { c->last_ptrs[k] = ptrs[k]; c->last_gens[k] = gens[k]; }
+  for (int k = 0; k < kPeerArrays; k++) { c->last_ptrs[k] = ptrs[k]; c->last_gens[k] = gens[k]; }
   c->ipc_valid = true;
   }
   // where my send segments land in each peer's community array: its lnv + its receive offset for me
@@ -466,6 +477,44 @@ int launch_scan(mvgpu_ctx *c, const ScanParams &sp, bool first) {
 int exchange_ghosts(mvgpu_ctx *c, int32_t *comm);
 int final_in_caller_order(mvgpu_ctx *c);
 
+// "every rank's stream has reached this point" on the run's data plane (comm_mode): one-rank runs are stream ordered
+int run_barrier(mvgpu_ctx *c) {
+  if (c->nranks == 1) return 0;
+  if (c->opt_comm_mode == 1) {
+    k_p2p_barrier<<<1, 32, 0, c->stream>>>(c->pp, ++c->p2p_epoch);
+    c->tm.kernel_launches++;
+    CK(cudaGetLastError());
+    return 0;
+  }
+  return coll_barrier(c);
+}
+
+// Warm start: comm_a := the initial assignment in internal ids (ghost slots by the usual exchange), Comm records := its
+// aggregates.  Runs after setup_peers, over k_vertex_init's singleton state (degrees, self loops, 1/(2m) stay).
+int warm_init(mvgpu_ctx *c) {
+  cudaStream_t s = c->stream;
+  const int lnv = (int)c->lnv, nsm = c->num_sms;
+  // every rank's inv is written and its update arrays are zeroed (k_vertex_init) before a peer reads or adds to them
+  if (c->nranks > 1) TRY(coll_barrier(c));
+  WarmInv m;
+  memset(&m, 0, sizeof m);
+  for (int r = 0; r < c->nranks; r++) m.inv[r] = c->relabel ? c->peer_inv[r] : nullptr;
+  k_warm_map<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->init_comm.p, c->relabel ? c->inv.p : nullptr, c->pt, m, c->comm_a.p);
+  c->tm.kernel_launches++;
+  if (c->nranks > 1) TRY(exchange_ghosts(c, c->comm_a.p));
+  if (c->unit) k_warm_comm_unit<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->comm_a.p, c->a_rowptr, c->pt);
+  else k_warm_comm_w<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->comm_a.p, c->vdeg.p, c->pt);
+  c->tm.kernel_launches++;
+  TRY(run_barrier(c));                        // all deltas have landed
+  CK(cudaMemsetAsync(c->acc.p, 0, sizeof(Acc), s));
+  if (c->unit) k_warm_fold_unit<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->cdeg.p, c->csize.p, c->upd.p, c->acc.p);
+  else k_warm_fold_w<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->cinfo_w.p, c->usize.p, c->udeg.p);
+  c->tm.kernel_launches++;
+  TRY(run_barrier(c));                        // no scan reads or updates a record before its owner has folded it
+  CK(cudaGetLastError());
+  return 0;
+}
+
 // ---- setup: reference-format arrays -> compact graph, ghosts, init ------------------------------
 int setup_run(mvgpu_ctx *c) {
   cudaStream_t s = c->stream;
@@ -475,6 +524,7 @@ int setup_run(mvgpu_ctx *c) {
   Scalars h;
   CK(cudaMemsetAsync(d_sc, 0, sizeof(Scalars), s));
   const long long lnv = c->lnv, lne = c->lne;
+  c->warm_run = c->have_init;
 
   // pass 1 over the edges: unit weights? how many non-owned tails? (+ input validation).  The compact upload
   // format has answered all of that on the host already.
@@ -513,12 +563,15 @@ int setup_run(mvgpu_ctx *c) {
     // mapping before the owner frees the block, so that is agreed on here and done collectively
     const size_t need_v = (size_t)lnv, need_s = (size_t)(lnv + (long long)h.st.nremote);
     const bool grow = c->ipc_valid && ((c->cdeg.p && c->cdeg.cap < need_v) || (c->cinfo_w.p && c->cinfo_w.cap < need_v) ||
-                                       (c->lab.p && c->lab.cap < need_v) || c->comm_a.cap < need_s || c->comm_b.cap < need_s);
-    long long hv[4] = {unit ? 0 : 1, lne, input_err.empty() ? 0 : 1, grow ? 1 : 0};
-    TRY(coll_allreduce_i64(c, hv, 4, false));
+                                       (c->lab.p && c->lab.cap < need_v) || (c->inv.p && c->inv.cap < need_v) ||
+                                       c->comm_a.cap < need_s || c->comm_b.cap < need_s);
+    long long hv[5] = {unit ? 0 : 1, lne, input_err.empty() ? 0 : 1, grow ? 1 : 0, c->warm_run ? 1 : 0};
+    TRY(coll_allreduce_i64(c, hv, 5, false));
     unit = hv[0] == 0;
     ne_global = hv[1];
     if (hv[2] && input_err.empty()) input_err = "another rank rejected its shard";
+    if (input_err.empty() && hv[4] != 0 && hv[4] != c->nranks)
+      input_err = "ranks disagree on the initial assignment: every rank or none must set one";
     if (hv[3]) {
       for (void *q : c->ipc_opened) cudaIpcCloseMemHandle(q);
       c->ipc_opened.clear();
@@ -759,8 +812,8 @@ int setup_run(mvgpu_ctx *c) {
                                                                nullptr, c->self_d.p, &d_sc->total_weight, &d_sc->has_self, 0, nullptr, nullptr);
   c->tm.kernel_launches++;
   // ghosts start in their own (internal) singleton community, which only the owner knows after renumbering:
-  // fetch it with the same all-to-all-v the iterations use
-  if (c->nranks > 1) TRY(exchange_ghosts(c, c->comm_a.p));
+  // fetch it with the same all-to-all-v the iterations use (a warm run fills comm_a in warm_init instead)
+  if (c->nranks > 1 && !c->warm_run) TRY(exchange_ghosts(c, c->comm_a.p));
 
   // high-degree vertices
   // largest degree the tile kernels take: one staging buffer (minus the 16-byte alignment slack of the bulk copies)
@@ -808,6 +861,7 @@ int setup_run(mvgpu_ctx *c) {
     if (!c->p2p_zeroed) { CK(cudaMemsetAsync(c->p2p.p, 0, sizeof(P2PState), s)); CK(cudaStreamSynchronize(s)); c->p2p_zeroed = true; }
   }
   TRY(setup_peers(c, c->unit ? 1 : 0));
+  if (c->warm_run) TRY(warm_init(c));
   c->tm.unit_weight = c->unit ? 1 : 0;
   c->scan_has_self = has_self;
   c->scan_heavy_deg = (int)heavy_deg;
@@ -864,6 +918,7 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   const size_t ev_iter0 = ev;
   double prevMod = lower, currMod = -1.0;
   int numIters = 0, auto_choice = 4;
+  c->converged = 1;
   const int fold_grid = grid_for(c->lnv, 256, c->num_sms, 8);
   for (;;) {                                                   // dspl.hpp:1338
     if (numIters >= c->opt_max_iters) return fail("max_iters reached without convergence");
@@ -884,7 +939,8 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
       if (numIters == 3) c->scan_kernel = 5;
       else if (numIters >= 5) c->scan_kernel = auto_choice;
     }
-    TRY(launch_scan(c, sp, numIters == 1 && c->simple_sorted && c->opt_first_iter && c->opt_scan_variant >= 4 && !c->f32));
+    // (not on a warm run: its communities are not singletons)
+    TRY(launch_scan(c, sp, numIters == 1 && c->simple_sorted && c->opt_first_iter && c->opt_scan_variant >= 4 && !c->f32 && !c->warm_run));
     CK(cudaEventRecord(e1, s));
     const bool p2p = c->nranks > 1 && c->opt_comm_mode == 1;
     if (c->nranks > 1) {
@@ -971,6 +1027,7 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
     prevMod = currMod;
     if (prevMod < lower) prevMod = lower;                      // dspl.hpp:1404-1406
     std::swap(cur, tgt);                                       // rotation (dspl.hpp:1408-1422) is a pointer swap
+    if (c->opt_stop_after > 0 && numIters == c->opt_stop_after) { c->converged = 0; break; }   // checkpoint: resume with lower = prevMod
   }
   cudaEvent_t e_end = get_event(c, ev++);
   CK(cudaEventRecord(e_end, s));
@@ -1516,6 +1573,31 @@ int mvgpu_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters, double 
   return run_louvain(c, lower, thresh, iters, modularity);
 }
 
+int mvgpu_set_initial_communities(mvgpu_ctx *c, const int64_t *comm) {
+  if (!c) return fail("null argument");
+  if (!comm) { c->have_init = false; return 0; }
+  if (!c->have_graph) return fail("mvgpu_set_initial_communities: no shard yet (upload, attach or generate one first)");
+  std::vector<int32_t> h((size_t)c->lnv);
+  for (long long i = 0; i < c->lnv; i++) {
+    if (comm[i] < 0 || comm[i] >= c->nv_global)
+      return fail("mvgpu_set_initial_communities: community id " + std::to_string((long long)comm[i]) + " of local vertex " +
+                  std::to_string(i) + " outside [0, nv)");
+    h[i] = (int32_t)comm[i];
+  }
+  CK(cudaSetDevice(c->device));
+  TRY(c->init_comm.ensure(c->lnv));
+  if (c->lnv) CK(cudaMemcpy(c->init_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice));
+  c->have_init = true;
+  return 0;
+}
+
+int mvgpu_get_converged(mvgpu_ctx *c, int *converged) {
+  if (!c || !converged) return fail("null argument");
+  if (!c->d_final) return fail("no result yet");
+  *converged = c->converged;
+  return 0;
+}
+
 int mvgpu_get_communities_device(mvgpu_ctx *c, const int32_t **d_out) {
   if (!c || !c->d_final) return fail("no result yet");
   TRY(final_in_caller_order(c));
@@ -1579,6 +1661,7 @@ int mvgpu_set_option(mvgpu_ctx *c, const char *name, int64_t value) {
   else if (n == "compact_upload") c->opt_compact_upload = (int)value;
   else if (n == "host_threads") c->opt_host_threads = (int)value;
   else if (n == "first_iter") c->opt_first_iter = value != 0;
+  else if (n == "stop_after") { if (value < 0) return fail("stop_after < 0"); c->opt_stop_after = value; }
   else if (n == "upload_chunk") { if (value < 256 || (value & 3)) return fail("upload_chunk must be a multiple of 4, >= 256"); c->opt_upload_chunk = value; }
   else if (n == "host_transport") {
     if ((c->comm || c->hc.is_open()) && c->opt_host_transport != (value != 0)) return fail("host_transport must be set before mvgpu_comm_init");
@@ -1693,6 +1776,7 @@ int mvgpu_upload_shard32(mvgpu_ctx *c, int32_t nv_global, const int32_t *parts, 
 int mvgpu_louvain32(mvgpu_ctx *c, float lower, float thresh, int *iters, float *modularity) {
   if (!c || !iters || !modularity) return fail("null argument");
   if (!c->f32) return fail("mvgpu_louvain32 needs a shard uploaded with mvgpu_upload_shard32");
+  if (c->have_init || c->opt_stop_after) return fail("mvgpu_louvain32 supports neither an initial assignment nor stop_after");
   double mod = 0.0;
   TRY(run_louvain(c, (double)lower, (double)thresh, iters, &mod));
   *modularity = (float)mod;

@@ -30,7 +30,8 @@ EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_dest
            "mvgpu_comm_init", "mvgpu_upload_shard", "mvgpu_attach_shard_device", "mvgpu_generate_rgg_shard", "mvgpu_generate_rgg_shard_ex",
            "mvgpu_download_shard", "mvgpu_louvain",
            "mvgpu_get_communities", "mvgpu_get_communities_device", "mvgpu_upload_shard32", "mvgpu_louvain32", "mvgpu_get_communities32", "mvgpu_set_option", "mvgpu_get_trace",
-           "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method"]
+           "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method",
+           "mvgpu_set_initial_communities", "mvgpu_get_converged"]
 
 _lib = None
 
@@ -56,6 +57,8 @@ def lib():
         L.mvgpu_download_shard.argtypes = [vp, vp, vp]
         L.mvgpu_louvain.argtypes = [vp, dbl, dbl, ctypes.POINTER(ci), ctypes.POINTER(dbl)]
         L.mvgpu_get_communities.argtypes = [vp, vp]
+        L.mvgpu_set_initial_communities.argtypes = [vp, vp]
+        L.mvgpu_get_converged.argtypes = [vp, ctypes.POINTER(ci)]
         L.mvgpu_upload_shard32.argtypes = [vp, ctypes.c_int32, vp, ctypes.c_int32, ctypes.c_int32, vp, vp]
         L.mvgpu_louvain32.argtypes = [vp, ctypes.c_float, ctypes.c_float, ctypes.POINTER(ci), ctypes.POINTER(ctypes.c_float)]
         L.mvgpu_get_communities32.argtypes = [vp, vp]
@@ -177,6 +180,26 @@ class LouvainGPU:
         mod = ctypes.c_double(0.0)
         _ck(lib().mvgpu_louvain(self._h, lower, thresh, ctypes.byref(iters), ctypes.byref(mod)))
         return mod.value, iters.value
+
+    def set_initial_communities(self, comm):
+        """Start every later louvain() on this shard from `comm` (lnv global community ids in [0, nv), caller's vertex
+        numbering, e.g. what communities() returned) instead of singletons; None clears it.  A new upload / attach /
+        generate clears it too.  Resuming a run stopped by the stop_after option from its communities() with lower = its
+        modularity continues that run exactly."""
+        if comm is None:
+            _ck(lib().mvgpu_set_initial_communities(self._h, None))
+            return
+        comm = np.ascontiguousarray(comm, dtype=np.int64)
+        if comm.ndim != 1 or comm.size != self.lnv:
+            raise ValueError(f"initial assignment has {comm.size} entries, the shard has lnv = {self.lnv}")
+        buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
+        _ck(lib().mvgpu_set_initial_communities(self._h, buf.ctypes.data))
+
+    def converged(self):
+        """True if the last louvain() ended on the exit test, False if the stop_after option ended it first."""
+        v = ctypes.c_int(0)
+        _ck(lib().mvgpu_get_converged(self._h, ctypes.byref(v)))
+        return bool(v.value)
 
     def communities(self, out=None):
         """currComm of this rank's vertices (global community ids).  `out`: optional preallocated int64 array
