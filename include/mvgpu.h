@@ -114,6 +114,33 @@ int mvgpu_set_initial_communities(mvgpu_ctx *ctx, const int64_t *comm);
 /* 1 if the last mvgpu_louvain ended on the reference's exit test, 0 if "stop_after" ended it first. */
 int mvgpu_get_converged(mvgpu_ctx *ctx, int *converged);
 
+/* ---- quality of an assignment (DESIGN.md §3.10) ---------------------------------------------------------------------
+ * The modularity mvgpu_louvain returns is the reference's mixed quantity: in iteration k the intra-community weight is
+ * measured on the assignment the scan read and sum(a_c^2) on the one it wrote.  mvgpu_evaluate_communities gives the
+ * modularity Q of one assignment X.  Every field is global (all ranks) and identical on every rank. */
+typedef struct {
+  double modularity;   /* Q(X) = e_in*c - (a2*c)*c, rounded like the run's currMod, signed (no fabs) */
+  double e_in;         /* sum over vertices i, edges (i,j) with X(j) = X(i) of w_ij (self-loop records count once each) */
+  double a2;           /* sum over communities of a_c^2, a_c = sum of the degrees of c's members */
+  double constant;     /* c = 1/(2m), as a run computes it */
+  int64_t communities; /* non-empty communities */
+  int64_t singletons;  /* communities of exactly one vertex */
+  int64_t max_size;    /* vertices in the largest community */
+  double eval_s;       /* device time of the evaluation (CUDA events on the context's stream) */
+} mvgpu_quality;
+/* Collective.  comm: lnv community ids in [0, nv) in the caller's vertex numbering, the form
+ * mvgpu_set_initial_communities takes; NULL evaluates the assignment the last mvgpu_louvain on this shard returned (an
+ * error if there is none).  A bad id on any rank, or ranks that disagree on NULL, fail the call on every rank.  Leaves
+ * everything the last run reports (communities, trace, timings, constant, converged) and the initial assignment as they
+ * were.  Not for shards uploaded with mvgpu_upload_shard32. */
+int mvgpu_evaluate_communities(mvgpu_ctx *ctx, const int64_t *comm, mvgpu_quality *out);
+/* Per community of the last evaluation, lnv entries each (any may be NULL): entry s describes community
+ * parts[rank] + s (caller numbering): its number of vertices, its volume a_c and its share of e_in.  Empty: zeros. */
+int mvgpu_get_community_stats(mvgpu_ctx *ctx, int64_t *size, double *volume, double *internal);
+/* Per vertex of the last evaluation, lnv entries: the rank of its community among the non-empty community ids in
+ * ascending caller id, in [0, communities); independent of the rank count and of the locality renumbering. */
+int mvgpu_get_compact_communities(mvgpu_ctx *ctx, int64_t *out);
+
 /* currComm of this rank's vertices at exit (global community ids), lnv entries. */
 int mvgpu_get_communities(mvgpu_ctx *ctx, int64_t *out);
 /* Same values left in device memory (int32 global ids); valid until the next mvgpu_louvain. */

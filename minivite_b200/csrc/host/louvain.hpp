@@ -25,6 +25,9 @@ struct GpuRankContext {
   const std::vector<GraphElem> *init_comm = nullptr;   // -i: starting assignment of this rank's vertices (global ids)
   int stop_after = 0;                                  // -k: stop after that many accepted iterations (0 = off)
   bool stopped = false;                                // the run ended by stop_after, not by the exit test
+  bool quality = false;                                // -q: evaluate the returned assignment after the run
+  const std::vector<GraphElem> *eval_comm = nullptr;   // -E: evaluate this assignment instead of running the phase
+  mvgpu_quality q{};                                   // -q / -E: the evaluation (global values)
 };
 
 [[noreturn]] inline void mv_abort(const std::string &where) {
@@ -63,6 +66,17 @@ inline void mv_apply_warm_start(mvgpu_ctx *ctx, const GpuRankContext &rc) {
   if (rc.init_comm && mvgpu_set_initial_communities(ctx, rc.init_comm->data())) mv_abort("mvgpu_set_initial_communities");
   if (rc.stop_after && mvgpu_set_option(ctx, "stop_after", rc.stop_after)) mv_abort("stop_after");
 }
+// -E: evaluate the given assignment and run no Louvain phase (true: done, the caller returns)
+inline bool mv_evaluate_only(mvgpu_ctx *ctx, GpuRankContext &rc) {
+  if (!rc.eval_comm) return false;
+  if (mvgpu_evaluate_communities(ctx, rc.eval_comm->data(), &rc.q)) mv_abort("mvgpu_evaluate_communities");
+  mvgpu_destroy(ctx);
+  return true;
+}
+// -q: evaluate the assignment the run returned
+inline void mv_evaluate_run(mvgpu_ctx *ctx, GpuRankContext &rc) {
+  if (rc.quality && mvgpu_evaluate_communities(ctx, nullptr, &rc.q)) mv_abort("mvgpu_evaluate_communities");
+}
 inline void mv_read_converged(mvgpu_ctx *ctx, GpuRankContext &rc) {
   int conv = 1;
   if (mvgpu_get_converged(ctx, &conv)) mv_abort("mvgpu_get_converged");
@@ -100,9 +114,11 @@ inline GraphWeight distLouvainMethod(const int me, const int nprocs, const Graph
                          dg.edge_list_.data()))
     mv_abort("mvgpu_upload_shard");
   mv_apply_warm_start(ctx, rc);
+  if (mv_evaluate_only(ctx, rc)) return lower;
   double mod = 0.0;
   for (int rep = mv_env_repeat(); rep > 0; rep--)
     if (mvgpu_louvain(ctx, lower, thresh, &iters, &mod)) mv_abort("mvgpu_louvain");
+  mv_evaluate_run(ctx, rc);
   mvgpu_get_timings(ctx, &rc.timings);
   mv_read_converged(ctx, rc);
   mv_print_scan_times(ctx, me);
@@ -139,9 +155,11 @@ inline GraphWeight distLouvainMethodOnDeviceRGG(const int me, const int nprocs, 
   lne = lne64;
   mv_apply_warm_start(ctx, rc);
   before_louvain();
+  if (mv_evaluate_only(ctx, rc)) return lower;
   double mod = 0.0;
   for (int rep = mv_env_repeat(); rep > 0; rep--)
     if (mvgpu_louvain(ctx, lower, thresh, &iters, &mod)) mv_abort("mvgpu_louvain");
+  mv_evaluate_run(ctx, rc);
   mvgpu_get_timings(ctx, &rc.timings);
   mv_read_converged(ctx, rc);
   mv_print_scan_times(ctx, me);

@@ -10,6 +10,8 @@
 //            -D generate the RGG on the GPU (same graph; with -n, also -w, -l and -p; without -s)
 //            -i <prefix> start from the communities an earlier -o <prefix> wrote   -k <n> stop after n accepted
 //            iterations (prints STOPPED iters=<n> prevMod=<v>)   -L <v> starting `lower` (default -1; resume: -L <v>)
+//            -q evaluate the returned assignment (prints QUALITY mod=.. e=.. a2=.. communities=.. singletons=.. maxsize=..)
+//            -E <prefix> evaluate the communities an earlier -o <prefix> wrote, without a Louvain phase (prints QUALITY)
 #include <getopt.h>
 #include <sys/mman.h>
 #include <sys/wait.h>
@@ -29,13 +31,14 @@
 #include "louvain.hpp"
 #include "rgg.hpp"
 
-static std::string inputFileName, dumpPrefix, initPrefix;
+static std::string inputFileName, dumpPrefix, initPrefix, evalPrefix;
 static int stopAfter = 0;
 static GraphWeight lowerStart = -1.0;
 static int me = 0, nprocs = 1;
 static int ranksPerNode = 1;
 static GraphElem nvRGG = 0;
-static bool generateGraph = false, readBalanced = false, showGraph = false, traceIters = false, deviceGenerate = false;
+static bool generateGraph = false, readBalanced = false, showGraph = false, traceIters = false, deviceGenerate = false,
+            evalQuality = false;
 static GraphWeight randomEdgePercent = 0.0;
 static bool randomNumberLCG = false, isUnitEdgeWeight = true;
 static GraphWeight threshold = 1.0E-6;
@@ -84,7 +87,7 @@ static long long reduce_sum_ll(long long v) {
 
 static void parseCommandLine(const int argc, char *const argv[]) {
   int ret;
-  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:")) != -1) {
+  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:")) != -1) {
     switch (ret) {
       case 'f': inputFileName.assign(optarg); break;
       case 'b': readBalanced = true; break;
@@ -102,6 +105,8 @@ static void parseCommandLine(const int argc, char *const argv[]) {
       case 'i': initPrefix.assign(optarg); break;
       case 'k': stopAfter = atoi(optarg); break;
       case 'L': lowerStart = atof(optarg); break;
+      case 'q': evalQuality = true; break;
+      case 'E': evalPrefix.assign(optarg); break;
       default: assert(0 && "Option not recognized!!!"); break;
     }
   }
@@ -126,6 +131,9 @@ static void parseCommandLine(const int argc, char *const argv[]) {
     std::cerr << "-D (generate the RGG on the GPU) needs -n and excludes -s." << std::endl; exit(99);
   }
   if (stopAfter < 0) { std::cerr << "-k needs a number of iterations >= 0." << std::endl; exit(99); }
+  if (!evalPrefix.empty() && (!initPrefix.empty() || !dumpPrefix.empty() || stopAfter)) {
+    std::cerr << "-E runs no Louvain phase: it excludes -i, -o and -k." << std::endl; exit(99);
+  }
 }
 
 int main(int argc, char *argv[]) {
@@ -228,27 +236,35 @@ int main(int argc, char *argv[]) {
     memcpy(rc.unique_id, shm->unique_id, sizeof rc.unique_id);
   }
 
-  // -i: this rank's slice of an earlier run's -o dump ({base, lnv} header, then lnv global community ids)
-  std::vector<GraphElem> initComm;
-  if (!initPrefix.empty()) {
+  // -i / -E: this rank's slice of an earlier run's -o dump ({base, lnv} header, then lnv global community ids)
+  auto read_assignment = [&](const char *flag, const std::string &prefix, std::vector<GraphElem> &comm) {
     const long long want_base = deviceGenerate ? (long long)(nvRGG / nprocs) * me : (long long)g->get_base(me);
     const long long want_lnv = deviceGenerate ? (long long)(nvRGG / nprocs) : (long long)g->get_lnv();
-    const std::string fn = initPrefix + "." + std::to_string(me);
+    const std::string fn = prefix + "." + std::to_string(me);
     FILE *f = fopen(fn.c_str(), "rb");
     long long hdr[2] = {-1, -1};
     bool ok = f && fread(hdr, 8, 2, f) == 2 && hdr[0] == want_base && hdr[1] == want_lnv;
     if (ok) {
-      initComm.resize((size_t)want_lnv);
-      ok = fread(initComm.data(), sizeof(GraphElem), initComm.size(), f) == initComm.size();
+      comm.resize((size_t)want_lnv);
+      ok = fread(comm.data(), sizeof(GraphElem), comm.size(), f) == comm.size();
     }
     if (f) fclose(f);
     if (!ok)
-      fprintf(stderr, "[miniVite_b200] -i %s: cannot read %s or its header {base %lld, lnv %lld} does not match this rank's "
-              "shard {base %lld, lnv %lld}\n", initPrefix.c_str(), fn.c_str(), hdr[0], hdr[1], want_base, want_lnv);
+      fprintf(stderr, "[miniVite_b200] %s %s: cannot read %s or its header {base %lld, lnv %lld} does not match this rank's "
+              "shard {base %lld, lnv %lld}\n", flag, prefix.c_str(), fn.c_str(), hdr[0], hdr[1], want_base, want_lnv);
     if (reduce_sum_ll(ok ? 0 : 1)) abort_all(99);       // every rank leaves, not only the one with the bad file
+  };
+  std::vector<GraphElem> initComm, evalComm;
+  if (!initPrefix.empty()) {
+    read_assignment("-i", initPrefix, initComm);
     rc.init_comm = &initComm;
   }
+  if (!evalPrefix.empty()) {
+    read_assignment("-E", evalPrefix, evalComm);
+    rc.eval_comm = &evalComm;
+  }
   rc.stop_after = stopAfter;
+  rc.quality = evalQuality;
 
   GraphWeight currMod = lowerStart;
   std::vector<GraphElem> ssizes, rsizes, svdata, rvdata;
@@ -280,6 +296,9 @@ int main(int argc, char *argv[]) {
   const double total = wtime() - t1;
   const double tot_time = reduce_sum(total);
   const double dev_time = reduce_sum(rc.timings.total_s);
+  if (me == 0 && (evalQuality || !evalPrefix.empty()))
+    fprintf(stderr, "QUALITY mod=%.17g e=%.17g a2=%.17g communities=%ld singletons=%ld maxsize=%ld\n", rc.q.modularity,
+            rc.q.e_in, rc.q.a2, (long)rc.q.communities, (long)rc.q.singletons, (long)rc.q.max_size);
 
   if (traceIters && me == 0)
     for (size_t k = 0; k < rc.iter_trace.size(); k++)
@@ -293,7 +312,7 @@ int main(int argc, char *argv[]) {
     fwrite(comm.data(), sizeof(GraphElem), comm.size(), f);
     fclose(f);
   }
-  if (me == 0) {
+  if (me == 0 && evalPrefix.empty()) {            // (-E ran no Louvain phase: nothing to report)
     const double avgt = tot_time / nprocs, avgd = dev_time / nprocs;
     if (!generateGraph) {
       std::cout << "-------------------------------------------------------" << std::endl;

@@ -1330,4 +1330,93 @@ __global__ void __launch_bounds__(256) k_warm_fold_w(int lnv, CommW *cinfo_w, lo
   }
 }
 
+// ----------------------------------------------------------------------------------------------
+// Quality of an assignment (mvgpu_evaluate_communities, DESIGN.md §3.10).  warm_init has built the Comm records of the
+// assignment X and cur = X on every slot (ghosts included); evaluation runs without the locality renumbering, so
+// internal ids are caller ids and owned slot s is caller community parts[rank] + s.
+// ----------------------------------------------------------------------------------------------
+struct QualPeers {                                  // every rank's evaluation arrays (peer mappings for other ranks)
+  double *internal[kMaxRanks];                      // per owned community: its share of e_in (unit path: uint64 counts
+                                                    // until k_q_stats converts them in place)
+  const int32_t *rank[kMaxRanks];                   // per owned community: exclusive prefix sum of the non-empty flags
+  long long off[kMaxRanks];                         // non-empty communities owned by lower ranks
+};
+
+// e_in: per vertex the weight of its edges whose tail is in its own community (self-loop records included, once per
+// record; the reference's counter[0], dspl.hpp:318), counted in integers on the unit path and summed in fp64 in edge
+// order otherwise; added to the community's owner record and to acc->le_u / le_d
+template <bool UNIT>
+__global__ void __launch_bounds__(256) k_q_internal(int lnv, const uint32_t *rowptr, const int32_t *tails, const double *weights,
+                                                    const int32_t *cur, PeerTable pt, QualPeers q, Acc *acc) {
+  unsigned long long su = 0;
+  double sd = 0.0;
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) {
+    const int cv = cur[v];
+    const uint32_t e1 = rowptr[v + 1];
+    unsigned long long cu = 0;
+    double cd = 0.0;
+    for (uint32_t e = rowptr[v]; e < e1; e++)
+      if (cur[tails[e]] == cv) {
+        if (UNIT) cu++;
+        else cd += weights[e];
+      }
+    if (UNIT ? cu != 0 : cd != 0.0) {
+      int o; long long idx;
+      locate_remote(pt, cv, o, idx);
+      if (UNIT) atomicAdd(reinterpret_cast<unsigned long long *>(q.internal[o]) + idx, cu);
+      else atomicAdd(q.internal[o] + idx, cd);
+    }
+    su += cu; sd += cd;
+  }
+  if (UNIT) {
+    su = warp_sum(su);
+    if ((threadIdx.x & 31) == 0 && su) atomicAdd(&acc->le_u, su);
+  } else {
+    sd = warp_sum(sd);
+    if ((threadIdx.x & 31) == 0 && sd != 0.0) atomicAdd(&acc->le_d, sd);
+  }
+}
+
+// per owned community: size, volume (a_c) and internal weight as int64 / fp64 for mvgpu_get_community_stats, the
+// non-empty flag the compaction scans (flag[lnv] = 0 so that the exclusive sum ends in the count), and the number of
+// singletons / the largest size (agg[0] / agg[1])
+template <bool UNIT>
+__global__ void __launch_bounds__(256) k_q_stats(int lnv, const uint32_t *cdeg, const int32_t *csize, const CommW *cinfo_w,
+                                                 double *internal, long long *size_out, double *vol_out, int32_t *flag,
+                                                 unsigned long long *agg) {
+  unsigned long long single = 0, mx = 0;
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < lnv; s += gridDim.x * blockDim.x) {
+    long long sz;
+    double vol;
+    if (UNIT) {
+      sz = csize[s]; vol = (double)cdeg[s];
+      internal[s] = (double)reinterpret_cast<const unsigned long long *>(internal)[s];
+    } else {
+      const CommW c = cinfo_w[s];
+      sz = c.size; vol = c.degree;
+    }
+    size_out[s] = sz; vol_out[s] = vol;
+    flag[s] = sz != 0;
+    single += sz == 1;
+    mx = max(mx, (unsigned long long)sz);
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) flag[lnv] = 0;
+  single = warp_sum(single);
+  for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) {
+    if (single) atomicAdd(&agg[0], single);
+    if (mx) atomicMax(&agg[1], mx);
+  }
+}
+
+// compact label of every vertex: the rank of its community among the non-empty ids in ascending caller id, read from
+// the owner's prefix sum (X holds caller ids in caller vertex order)
+__global__ void __launch_bounds__(256) k_q_labels(int lnv, const int32_t *X, PeerTable pt, QualPeers q, int32_t *out) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < lnv; i += gridDim.x * blockDim.x) {
+    int o; long long idx;
+    locate_remote(pt, X[i], o, idx);
+    out[i] = (int32_t)(q.off[o] + q.rank[o][idx]);
+  }
+}
+
 }  // namespace mv

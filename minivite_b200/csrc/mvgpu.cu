@@ -84,7 +84,7 @@ struct DevBuf {              // grow-only device buffer (allocations are cached 
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
-constexpr int kPeerArrays = 11;
+constexpr int kPeerArrays = 13;
 
 struct PeerBlob {            // what every rank publishes about its community arrays
   cudaIpcMemHandle_t h[kPeerArrays];
@@ -198,6 +198,14 @@ struct mvgpu_ctx {
   bool have_init = false;
   bool warm_run = false;               // the current / last run started from init_comm
   int converged = 1;                   // the last run ended on the exit test (0: stopped by stop_after)
+  // evaluation (mvgpu_evaluate_communities): q_internal and q_rank are peer-exported, the rest stays local
+  DevBuf<int32_t> eval_comm;           // the caller's assignment to evaluate (int32 caller ids)
+  DevBuf<double> q_internal, q_vol;
+  DevBuf<int32_t> q_rank, q_flag, q_lab;
+  DevBuf<long long> q_size;
+  QualPeers qp;
+  bool run_on_shard = false;           // final_orig holds a run's assignment of the current shard
+  bool eval_on_shard = false;          // the q_* arrays describe an evaluation of the current shard
   // results
   bool unit = true;
   bool f32 = false;                    // shard came through mvgpu_upload_shard32: float-build arithmetic (see mvgpu.h)
@@ -247,6 +255,7 @@ struct Scalars {
   unsigned long long tr2[2];
   long long counts[2 * kMaxRanks];
   unsigned long long span_sum, span_cnt;
+  unsigned long long q_agg[2];         // evaluation: singletons, largest community
 };
 
 // ---- setup-time collectives (a handful per run): NCCL on the library's stream, or the host transport ----------------
@@ -316,6 +325,7 @@ int coll_barrier(mvgpu_ctx *c) {
 int set_graph(mvgpu_ctx *c, long long nv_global, const int64_t *parts, long long lnv, long long lne) {
   if (c->nranks > kMaxRanks) return fail("too many ranks");
   c->have_init = false;                     // an initial assignment belongs to the shard it was given for
+  c->run_on_shard = c->eval_on_shard = false;   // so do a run's assignment and an evaluation
   if (nv_global < 0 || lnv < 0 || lne < 0) return fail("negative graph size");
   if (nv_global >= (1LL << 31)) return fail("nv_global >= 2^31: 32-bit community ids would overflow (not supported)");
   if (lne >= (1LL << 32)) return fail("lne >= 2^32 per shard: 32-bit edge offsets would overflow (not supported)");
@@ -340,16 +350,21 @@ int setup_peers(mvgpu_ctx *c, int unit) {
     pt.lab[0] = c->relabel ? c->lab.p : nullptr;
     pt.cdeg[0] = c->cdeg.p; pt.csize[0] = c->csize.p; pt.upd[0] = c->upd.p; pt.cinfo_w[0] = c->cinfo_w.p; pt.usize[0] = c->usize.p; pt.udeg[0] = c->udeg.p;
     c->peer_inv[0] = c->relabel ? c->inv.p : nullptr;
+    c->qp.internal[0] = c->q_internal.p; c->qp.rank[0] = c->q_rank.p;
     return 0;
   }
+  // the evaluation arrays are exported whenever they exist (an evaluation allocated them), so that alternating runs
+  // and evaluations reopen no mapping for them; lab / inv still differ between a renumbering run (exported) and an
+  // evaluation (never renumbers: NULL), so switching between those two reopens the mappings
   void *ptrs[kPeerArrays] = {unit ? (void *)c->cdeg.p : nullptr, unit ? (void *)c->csize.p : nullptr, unit ? (void *)c->upd.p : nullptr,
                     unit ? nullptr : (void *)c->cinfo_w.p, unit ? nullptr : (void *)c->usize.p,
                     unit ? nullptr : (void *)c->udeg.p, c->relabel ? (void *)c->lab.p : nullptr,
-                    (void *)c->comm_a.p, (void *)c->comm_b.p, (void *)c->p2p.p, c->relabel ? (void *)c->inv.p : nullptr};
+                    (void *)c->comm_a.p, (void *)c->comm_b.p, (void *)c->p2p.p, c->relabel ? (void *)c->inv.p : nullptr,
+                    (void *)c->q_internal.p, (void *)c->q_rank.p};
   if (c->peers_ready) return 0;            // same graph, same buffers: tables are still valid
   // IPC handles are expensive to (re)open: skip the exchange when no rank's buffers moved since the last one
   const unsigned gens[kPeerArrays] = {c->cdeg.gen, c->csize.gen, c->upd.gen, c->cinfo_w.gen, c->usize.gen, c->udeg.gen, c->lab.gen,
-                                      c->comm_a.gen, c->comm_b.gen, c->p2p.gen, c->inv.gen};
+                                      c->comm_a.gen, c->comm_b.gen, c->p2p.gen, c->inv.gen, c->q_internal.gen, c->q_rank.gen};
   long long changed = c->ipc_valid ? 0 : 1;
   for (int k = 0; k < kPeerArrays; k++) if (ptrs[k] != c->last_ptrs[k] || (ptrs[k] && gens[k] != c->last_gens[k])) changed = 1;
   TRY(coll_allreduce_i64(c, &changed, 1, true));
@@ -393,6 +408,7 @@ int setup_peers(mvgpu_ctx *c, int unit) {
     c->peer_comm[0][r] = (int32_t *)q[7]; c->peer_comm[1][r] = (int32_t *)q[8];
     c->pp.st[r] = (P2PState *)q[9];
     c->peer_inv[r] = (const int32_t *)q[10];
+    c->qp.internal[r] = (double *)q[11]; c->qp.rank[r] = (const int32_t *)q[12];
   }
   for (int k = 0; k < kPeerArrays; k++) { c->last_ptrs[k] = ptrs[k]; c->last_gens[k] = gens[k]; }
   c->ipc_valid = true;
@@ -489,9 +505,10 @@ int run_barrier(mvgpu_ctx *c) {
   return coll_barrier(c);
 }
 
-// Warm start: comm_a := the initial assignment in internal ids (ghost slots by the usual exchange), Comm records := its
-// aggregates.  Runs after setup_peers, over k_vertex_init's singleton state (degrees, self loops, 1/(2m) stay).
-int warm_init(mvgpu_ctx *c) {
+// Warm start: comm_a := the initial assignment `init` (caller ids) in internal ids (ghost slots by the usual exchange),
+// Comm records := its aggregates.  Runs after setup_peers, over k_vertex_init's singleton state (degrees, self loops,
+// 1/(2m) stay).
+int warm_init(mvgpu_ctx *c, const int32_t *init) {
   cudaStream_t s = c->stream;
   const int lnv = (int)c->lnv, nsm = c->num_sms;
   // every rank's inv is written and its update arrays are zeroed (k_vertex_init) before a peer reads or adds to them
@@ -499,7 +516,7 @@ int warm_init(mvgpu_ctx *c) {
   WarmInv m;
   memset(&m, 0, sizeof m);
   for (int r = 0; r < c->nranks; r++) m.inv[r] = c->relabel ? c->peer_inv[r] : nullptr;
-  k_warm_map<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->init_comm.p, c->relabel ? c->inv.p : nullptr, c->pt, m, c->comm_a.p);
+  k_warm_map<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, init, c->relabel ? c->inv.p : nullptr, c->pt, m, c->comm_a.p);
   c->tm.kernel_launches++;
   if (c->nranks > 1) TRY(exchange_ghosts(c, c->comm_a.p));
   if (c->unit) k_warm_comm_unit<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->comm_a.p, c->a_rowptr, c->pt);
@@ -515,8 +532,17 @@ int warm_init(mvgpu_ctx *c) {
   return 0;
 }
 
+// What an evaluation hands to setup_run: the assignment (caller ids, device) and what the caller side found wrong with
+// it, which joins the input agreement so that every rank fails together.
+struct EvalSetup {
+  const int32_t *X = nullptr;
+  bool given = false;                  // the caller passed an array (not NULL)
+  std::string err;
+};
+
 // ---- setup: reference-format arrays -> compact graph, ghosts, init ------------------------------
-int setup_run(mvgpu_ctx *c) {
+// ev != nullptr: setup for an evaluation -- warm init from ev->X, no locality renumbering, evaluation arrays allocated
+int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
   cudaStream_t s = c->stream;
   const int nsm = c->num_sms;
   TRY(c->scratch.ensure(sizeof(Scalars)));
@@ -524,7 +550,7 @@ int setup_run(mvgpu_ctx *c) {
   Scalars h;
   CK(cudaMemsetAsync(d_sc, 0, sizeof(Scalars), s));
   const long long lnv = c->lnv, lne = c->lne;
-  c->warm_run = c->have_init;
+  c->warm_run = ev ? true : c->have_init;
 
   // pass 1 over the edges: unit weights? how many non-owned tails? (+ input validation).  The compact upload
   // format has answered all of that on the host already.
@@ -554,6 +580,7 @@ int setup_run(mvgpu_ctx *c) {
   c->maxdeg = h.maxdeg;
   int unit = (!h.st.nonunit && !c->opt_force_weighted) ? 1 : 0;
   if (input_err.empty() && compact_in && !unit) input_err = "force_weighted needs the full edge records: set compact_upload=0";
+  if (input_err.empty() && ev) input_err = ev->err;
 
   // global agreement on the path + on 2m < 2^31 needs the total weight; the weight total itself comes
   // from the vertex-init kernel below, so first settle `unit` from the flags (ne bound checked after).
@@ -564,14 +591,18 @@ int setup_run(mvgpu_ctx *c) {
     const size_t need_v = (size_t)lnv, need_s = (size_t)(lnv + (long long)h.st.nremote);
     const bool grow = c->ipc_valid && ((c->cdeg.p && c->cdeg.cap < need_v) || (c->cinfo_w.p && c->cinfo_w.cap < need_v) ||
                                        (c->lab.p && c->lab.cap < need_v) || (c->inv.p && c->inv.cap < need_v) ||
-                                       c->comm_a.cap < need_s || c->comm_b.cap < need_s);
-    long long hv[5] = {unit ? 0 : 1, lne, input_err.empty() ? 0 : 1, grow ? 1 : 0, c->warm_run ? 1 : 0};
+                                       c->comm_a.cap < need_s || c->comm_b.cap < need_s ||
+                                       (ev && ((c->q_internal.p && c->q_internal.cap < need_v) ||
+                                               (c->q_rank.p && c->q_rank.cap < need_v + 1))));
+    const bool assigned = ev ? ev->given : c->warm_run;
+    long long hv[5] = {unit ? 0 : 1, lne, input_err.empty() ? 0 : 1, grow ? 1 : 0, assigned ? 1 : 0};
     TRY(coll_allreduce_i64(c, hv, 5, false));
     unit = hv[0] == 0;
     ne_global = hv[1];
-    if (hv[2] && input_err.empty()) input_err = "another rank rejected its shard";
+    if (hv[2] && input_err.empty()) input_err = ev ? "another rank rejected its shard or its assignment" : "another rank rejected its shard";
     if (input_err.empty() && hv[4] != 0 && hv[4] != c->nranks)
-      input_err = "ranks disagree on the initial assignment: every rank or none must set one";
+      input_err = ev ? "ranks disagree on the assignment to evaluate: every rank or none must pass NULL"
+                     : "ranks disagree on the initial assignment: every rank or none must set one";
     if (hv[3]) {
       for (void *q : c->ipc_opened) cudaIpcCloseMemHandle(q);
       c->ipc_opened.clear();
@@ -691,8 +722,9 @@ int setup_run(mvgpu_ctx *c) {
   c->lay_nregions = 0;
   c->lay_first_ran = false;
   {
-    int want = c->opt_reorder == 1 ? 1 : 0;
-    if (c->opt_reorder == 2 && lnv >= 65536) {
+    // (an evaluation makes one pass over the edges, which does not pay for a renumbering)
+    int want = !ev && c->opt_reorder == 1 ? 1 : 0;
+    if (!ev && c->opt_reorder == 2 && lnv >= 65536) {
       // auto: renumber when the given numbering has no locality (mean |tail - v| above lnv/64 on a vertex sample)
       k_span_sample<<<grid_for(lnv / 64 + 1, 256, nsm), 256, 0, s>>>((int)lnv, src_rowptr, src_tails, 64, &d_sc->span_sum, &d_sc->span_cnt);
       c->tm.kernel_launches++;
@@ -800,6 +832,10 @@ int setup_run(mvgpu_ctx *c) {
   else { TRY(c->cinfo_w.ensure(lnv)); TRY(c->usize.ensure(lnv)); TRY(c->udeg.ensure(lnv)); TRY(c->vdeg.ensure(lnv)); TRY(c->self_d.ensure(lnv)); }
   TRY(c->acc.ensure((size_t)c->opt_max_iters + 2));
   CK(cudaMemsetAsync(c->acc.p, 0, sizeof(Acc) * ((size_t)c->opt_max_iters + 2), s));
+  if (ev) {                                   // zeroed before warm_init's last barrier: no peer adds to it earlier
+    TRY(c->q_internal.ensure(lnv)); TRY(c->q_rank.ensure(lnv + 1));
+    CK(cudaMemsetAsync(c->q_internal.p, 0, sizeof(double) * lnv, s));
+  }
 
   if (c->unit)
     k_vertex_init<true><<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->base, c->a_rowptr, c->a_tails, nullptr, c->comm_a.p,
@@ -861,7 +897,7 @@ int setup_run(mvgpu_ctx *c) {
     if (!c->p2p_zeroed) { CK(cudaMemsetAsync(c->p2p.p, 0, sizeof(P2PState), s)); CK(cudaStreamSynchronize(s)); c->p2p_zeroed = true; }
   }
   TRY(setup_peers(c, c->unit ? 1 : 0));
-  if (c->warm_run) TRY(warm_init(c));
+  if (c->warm_run) TRY(warm_init(c, ev ? ev->X : c->init_comm.p));
   c->tm.unit_weight = c->unit ? 1 : 0;
   c->scan_has_self = has_self;
   c->scan_heavy_deg = (int)heavy_deg;
@@ -882,10 +918,16 @@ int exchange_ghosts(mvgpu_ctx *c, int32_t *comm) {
   return coll_alltoallv_dev(c, c->send_buf.p, c->scount, c->soff, comm + c->lnv, c->rcount, roff_slots, sizeof(int32_t));
 }
 
-int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, double *mod_out) {
+// a graph and, with several ranks, a communicator that carries the run's data plane
+int check_ready(mvgpu_ctx *c) {
   if (!c->have_graph) return fail("no graph uploaded");
   if (c->nranks > 1 && !c->comm && !c->hc.is_open()) return fail("mvgpu_comm_init has not been called");
   if (c->nranks > 1 && !c->comm && c->opt_comm_mode != 1) return fail("comm_mode=0 (NCCL data plane) needs the NCCL communicator: host_transport=1 supports comm_mode=1 only");
+  return 0;
+}
+
+int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, double *mod_out) {
+  TRY(check_ready(c));
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   memset(&c->tm, 0, sizeof c->tm);
@@ -1033,6 +1075,7 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   CK(cudaEventRecord(e_end, s));
   c->d_final = cur;
   c->final_ready = false;
+  c->run_on_shard = true;
   if (c->nranks > 1) {
     // the assignment in the caller's numbering needs the label arrays of the PEERS (a community may be owned by another
     // rank): resolve it now, while every rank is still inside this call, and leave together -- afterwards a rank may
@@ -1080,6 +1123,167 @@ int final_in_caller_order(mvgpu_ctx *c) {
 
 __global__ void k_widen(const int32_t *in, long long n, long long *out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = in[i];
+}
+
+// What the getters and mv_layout_readback report about the last run.  setup_run overwrites these, so an evaluation
+// keeps a copy and puts it back.
+struct RunReport {
+  mvgpu_timings tm;
+  double constant;
+  bool reordered, simple_sorted, unit, warm_run, lay_first_ran;
+  int relabel, lay_want, lay_stride, lay_unordered, lay_has_self;
+  long long lay_nregions, lay_span[2];
+  const int32_t *lay_tails;
+};
+RunReport save_report(const mvgpu_ctx *c) {
+  return {c->tm, c->constant, c->reordered, c->simple_sorted, c->unit, c->warm_run, c->lay_first_ran, c->relabel, c->lay_want,
+          c->lay_stride, c->lay_unordered, c->lay_has_self, c->lay_nregions, {c->lay_span[0], c->lay_span[1]}, c->lay_tails};
+}
+void restore_report(mvgpu_ctx *c, const RunReport &r) {
+  c->tm = r.tm; c->constant = r.constant; c->reordered = r.reordered; c->simple_sorted = r.simple_sorted; c->unit = r.unit;
+  c->warm_run = r.warm_run; c->lay_first_ran = r.lay_first_ran; c->relabel = r.relabel; c->lay_want = r.lay_want;
+  c->lay_stride = r.lay_stride; c->lay_unordered = r.lay_unordered; c->lay_has_self = r.lay_has_self;
+  c->lay_nregions = r.lay_nregions; c->lay_span[0] = r.lay_span[0]; c->lay_span[1] = r.lay_span[1]; c->lay_tails = r.lay_tails;
+}
+
+// ---- evaluation (DESIGN.md §3.10): after setup_run(ev), comm_a = X on every slot and the Comm records are X's -------
+int evaluate_pass(mvgpu_ctx *c, const int32_t *X, mvgpu_quality *out) {
+  cudaStream_t s = c->stream;
+  const int lnv = (int)c->lnv, nsm = c->num_sms;
+  Scalars *d_sc = reinterpret_cast<Scalars *>(c->scratch.p);
+  Acc *acc0 = c->acc.p;                        // warm_init left a2 (unit path) in record 0; e_in joins it there
+  if (!c->unit) {                              // the update arrays are zero after the warm fold: this only sums a_c^2
+    k_fold_w<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->cinfo_w.p, c->usize.p, c->udeg.p, acc0);
+    c->tm.kernel_launches++;
+  }
+  if (c->unit)
+    k_q_internal<true><<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->a_rowptr, c->a_tails, nullptr, c->comm_a.p, c->pt, c->qp, acc0);
+  else
+    k_q_internal<false><<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->a_rowptr, c->a_tails, c->a_weights, c->comm_a.p, c->pt, c->qp, acc0);
+  c->tm.kernel_launches++;
+  TRY(run_barrier(c));                         // every rank's internal-weight adds have landed in the owners' records
+  // e_in and a2, summed over the ranks in rank order like the run's modularity partials (dspl.hpp:441)
+  struct HostMail { Acc acc; double red2[2]; unsigned long long tr2[2]; unsigned int p2p_error; };
+  HostMail *mail = reinterpret_cast<HostMail *>(c->h_pin);
+  if (c->nranks > 1 && c->opt_comm_mode == 1) {
+    k_p2p_allreduce<<<1, 32, 0, s>>>(c->pp, ++c->p2p_epoch, acc0, c->unit ? 1 : 0, d_sc->red2, d_sc->tr2);
+    c->tm.kernel_launches++;
+    CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2, cudaMemcpyDeviceToHost, s));
+  } else if (c->nranks > 1) {
+    k_acc_to_double<<<1, 32, 0, s>>>(acc0, c->unit ? 1 : 0, d_sc->red2);
+    c->tm.kernel_launches++;
+    NK(g_nccl.AllReduce(d_sc->red2, d_sc->red2, 2, ncclDouble, ncclSum, c->comm, s));
+    CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2, cudaMemcpyDeviceToHost, s));
+  } else {
+    CK(cudaMemcpyAsync(&mail->acc, acc0, sizeof(Acc), cudaMemcpyDeviceToHost, s));
+  }
+  // per-community arrays, non-empty flags in owned slot order (= caller id order: no renumbering), their exclusive sum
+  TRY(c->q_flag.ensure(lnv + 1)); TRY(c->q_size.ensure(lnv)); TRY(c->q_vol.ensure(lnv)); TRY(c->q_lab.ensure(lnv));
+  CK(cudaMemsetAsync(d_sc->q_agg, 0, sizeof d_sc->q_agg, s));
+  if (c->unit)
+    k_q_stats<true><<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->cdeg.p, c->csize.p, nullptr, c->q_internal.p, c->q_size.p, c->q_vol.p,
+                                                            c->q_flag.p, d_sc->q_agg);
+  else
+    k_q_stats<false><<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, nullptr, nullptr, c->cinfo_w.p, c->q_internal.p, c->q_size.p, c->q_vol.p,
+                                                             c->q_flag.p, d_sc->q_agg);
+  size_t tb = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tb, c->q_flag.p, c->q_rank.p, lnv + 1, s);
+  TRY(c->cub_tmp.ensure(tb));
+  tb = c->cub_tmp.cap;
+  CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, c->q_flag.p, c->q_rank.p, lnv + 1, s));
+  c->tm.kernel_launches += 2;
+  int32_t nonempty = 0;
+  unsigned long long agg[2];
+  CK(cudaMemcpyAsync(&nonempty, c->q_rank.p + lnv, sizeof nonempty, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(agg, d_sc->q_agg, sizeof agg, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (c->nranks > 1 && c->opt_comm_mode == 1) {
+    unsigned int err = 0;
+    CK(cudaMemcpy(&err, &c->p2p.p->error, sizeof err, cudaMemcpyDeviceToHost));
+    if (err) return fail("peer-memory collective timed out (a peer rank is gone)");
+  }
+  // rank offsets of the compact labels: every rank's {non-empty, singletons, largest}; each rank's prefix sum is
+  // complete before it contributes, so the owners' arrays are final when the gather below reads them
+  std::vector<long long> all(3 * (size_t)c->nranks);
+  const long long mine[3] = {nonempty, (long long)agg[0], (long long)agg[1]};
+  if (c->nranks > 1) TRY(coll_allgather(c, mine, all.data(), sizeof mine));
+  else std::copy(mine, mine + 3, all.begin());
+  long long communities = 0, singletons = 0, max_size = 0;
+  for (int r = 0; r < c->nranks; r++) {
+    c->qp.off[r] = communities;
+    communities += all[3 * r]; singletons += all[3 * r + 1]; max_size = std::max(max_size, all[3 * r + 2]);
+  }
+  if (lnv > 0) {
+    k_q_labels<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, X, c->pt, c->qp, c->q_lab.p);
+    c->tm.kernel_launches++;
+  }
+  if (c->nranks > 1) {                         // no rank leaves while a peer still reads its prefix sums
+    TRY(run_barrier(c));
+    CK(cudaStreamSynchronize(s));
+  }
+  CK(cudaGetLastError());
+  const double e = c->nranks > 1 ? mail->red2[0] : (c->unit ? (double)mail->acc.le_u : mail->acc.le_d);
+  const double a2 = c->nranks > 1 ? mail->red2[1] : (c->unit ? (double)mail->acc.la2_u : mail->acc.la2_d);
+  const double cst = c->constant;              // run_louvain's rounding (dspl.hpp:447-448), without the fabs
+  volatile double term1 = e * cst;
+  volatile double term2a = a2 * cst;
+  volatile double term2 = term2a * cst;
+  out->modularity = term1 - term2;
+  out->e_in = e; out->a2 = a2; out->constant = cst;
+  out->communities = communities; out->singletons = singletons; out->max_size = max_size;
+  c->eval_on_shard = true;
+  return 0;
+}
+
+// collective: every rank calls it with an array or every rank with NULL.  caller_err: a finding of the caller's own
+// (a binding that could not build the array), which fails the call on every rank like a bad id
+int evaluate(mvgpu_ctx *c, const int64_t *comm, mvgpu_quality *out, const char *caller_err = nullptr) {
+  TRY(check_ready(c));
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  c->eval_on_shard = false;                    // the q_* arrays are rewritten from here on
+  // The last run's assignment in caller order is resolved while comm_a / comm_b still hold it (one-rank runs leave it
+  // unresolved; setup_run below overwrites comm_a), whatever is evaluated: communities(), get_communities_device and a
+  // later NULL evaluation read final_orig, which an evaluation never writes.
+  if (c->run_on_shard) TRY(final_in_caller_order(c));
+  EvalSetup ev;
+  ev.given = comm != nullptr;
+  // local findings are not returned here: they join setup_run's input agreement, so that every rank fails together
+  if (caller_err) ev.err = std::string("mvgpu_evaluate_communities: ") + caller_err;
+  else if (c->f32) ev.err = "mvgpu_evaluate_communities: not for a shard uploaded with mvgpu_upload_shard32";
+  else if (!comm && !c->run_on_shard) ev.err = "mvgpu_evaluate_communities: NULL evaluates the last mvgpu_louvain result, and there is none on this shard";
+  else if (comm) {
+    std::vector<int32_t> h((size_t)c->lnv);
+    for (long long i = 0; i < c->lnv && ev.err.empty(); i++) {
+      if (comm[i] < 0 || comm[i] >= c->nv_global)
+        ev.err = "mvgpu_evaluate_communities: community id " + std::to_string((long long)comm[i]) + " of local vertex " +
+                 std::to_string(i) + " outside [0, nv)";
+      h[i] = (int32_t)comm[i];
+    }
+    if (ev.err.empty()) {
+      TRY(c->eval_comm.ensure(c->lnv));
+      if (c->lnv) CK(cudaMemcpyAsync(c->eval_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice, s));
+      CK(cudaStreamSynchronize(s));
+      ev.X = c->eval_comm.p;
+    }
+  } else {
+    ev.X = c->final_orig.p;
+  }
+  const RunReport saved = save_report(c);
+  memset(&c->tm, 0, sizeof c->tm);
+  c->peers_ready = false;                      // the evaluation's tables differ from the run's (no labels, q arrays)
+  cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
+  int rc = cudaEventRecord(e0, s) == cudaSuccess ? 0 : fail("cudaEventRecord");
+  if (!rc) rc = setup_run(c, &ev);
+  if (!rc) rc = evaluate_pass(c, ev.X, out);
+  if (!rc && cudaEventRecord(e1, s) != cudaSuccess) rc = fail("cudaEventRecord");
+  if (!rc && cudaEventSynchronize(e1) != cudaSuccess) rc = fail("cudaEventSynchronize");
+  float ms = 0;
+  if (!rc && cudaEventElapsedTime(&ms, e0, e1) != cudaSuccess) rc = fail("cudaEventElapsedTime");
+  if (!rc) out->eval_s = ms * 1e-3;
+  restore_report(c, saved);
+  c->peers_ready = false;                      // the next run rebuilds its own tables
+  return rc;
 }
 
 }  // namespace
@@ -1195,6 +1399,7 @@ int mvgpu_create(mvgpu_ctx **out, int device, int rank, int nranks) {
   CK(cudaMallocHost(&c->h_pin, 4096));
   memset(&c->tm, 0, sizeof c->tm);
   memset(&c->pt, 0, sizeof c->pt);
+  memset(&c->qp, 0, sizeof c->qp);
   // developer knob: MVGPU_OPTIONS="name=value,name=value" presets options for every context of the process
   if (const char *e = getenv("MVGPU_OPTIONS")) {
     std::string all(e);
@@ -1239,6 +1444,8 @@ int mvgpu_destroy(mvgpu_ctx *c) {
   c->p2p.release();
   c->send_lid.release(); c->send_buf.release(); c->heavy_list.release(); c->hkeys.release(); c->hvals_i.release();
   c->hvals_d.release(); c->heavy_off.release();
+  c->eval_comm.release(); c->q_internal.release(); c->q_vol.release(); c->q_rank.release(); c->q_flag.release();
+  c->q_lab.release(); c->q_size.release();
   if (c->h_pin) cudaFreeHost(c->h_pin);
   if (c->stream) cudaStreamDestroy(c->stream);
   delete c;
@@ -1588,6 +1795,43 @@ int mvgpu_set_initial_communities(mvgpu_ctx *c, const int64_t *comm) {
   TRY(c->init_comm.ensure(c->lnv));
   if (c->lnv) CK(cudaMemcpy(c->init_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice));
   c->have_init = true;
+  return 0;
+}
+
+int mvgpu_evaluate_communities(mvgpu_ctx *c, const int64_t *comm, mvgpu_quality *out) {
+  if (!c || !out) return fail("null argument");
+  return evaluate(c, comm, out);
+}
+
+// Not in mvgpu.h: the Python binding's way into the collective when it cannot build the array (e.g. a wrong length), so
+// that the other ranks fail with it instead of waiting in the first setup all-reduce.
+int mv_evaluate_refused(mvgpu_ctx *c, const char *why, mvgpu_quality *out) {
+  if (!c || !out || !why) return fail("null argument");
+  return evaluate(c, nullptr, out, why);
+}
+
+int mvgpu_get_community_stats(mvgpu_ctx *c, int64_t *size, double *volume, double *internal) {
+  if (!c) return fail("null argument");
+  if (!c->eval_on_shard) return fail("no evaluation of this shard yet (mvgpu_evaluate_communities)");
+  CK(cudaSetDevice(c->device));
+  const size_t n = (size_t)c->lnv;
+  if (size && n) CK(cudaMemcpyAsync(size, c->q_size.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
+  if (volume && n) CK(cudaMemcpyAsync(volume, c->q_vol.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+  if (internal && n) CK(cudaMemcpyAsync(internal, c->q_internal.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+int mvgpu_get_compact_communities(mvgpu_ctx *c, int64_t *out) {
+  if (!c || !out) return fail("null argument");
+  if (!c->eval_on_shard) return fail("no evaluation of this shard yet (mvgpu_evaluate_communities)");
+  if (c->lnv == 0) return 0;
+  CK(cudaSetDevice(c->device));
+  TRY(c->wide.ensure(c->lnv));
+  k_widen<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(c->q_lab.p, c->lnv, c->wide.p);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * c->lnv, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
 

@@ -26,12 +26,22 @@ class Timings(ctypes.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class Quality(ctypes.Structure):
+    _fields_ = [("modularity", ctypes.c_double), ("e_in", ctypes.c_double), ("a2", ctypes.c_double),
+                ("constant", ctypes.c_double), ("communities", ctypes.c_int64), ("singletons", ctypes.c_int64),
+                ("max_size", ctypes.c_int64), ("eval_s", ctypes.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_destroy", "mvgpu_get_unique_id",
            "mvgpu_comm_init", "mvgpu_upload_shard", "mvgpu_attach_shard_device", "mvgpu_generate_rgg_shard", "mvgpu_generate_rgg_shard_ex",
            "mvgpu_download_shard", "mvgpu_louvain",
            "mvgpu_get_communities", "mvgpu_get_communities_device", "mvgpu_upload_shard32", "mvgpu_louvain32", "mvgpu_get_communities32", "mvgpu_set_option", "mvgpu_get_trace",
            "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method",
-           "mvgpu_set_initial_communities", "mvgpu_get_converged"]
+           "mvgpu_set_initial_communities", "mvgpu_get_converged", "mvgpu_evaluate_communities",
+           "mvgpu_get_community_stats", "mvgpu_get_compact_communities"]
 
 _lib = None
 
@@ -59,6 +69,10 @@ def lib():
         L.mvgpu_get_communities.argtypes = [vp, vp]
         L.mvgpu_set_initial_communities.argtypes = [vp, vp]
         L.mvgpu_get_converged.argtypes = [vp, ctypes.POINTER(ci)]
+        L.mvgpu_evaluate_communities.argtypes = [vp, vp, ctypes.POINTER(Quality)]
+        L.mv_evaluate_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(Quality)]
+        L.mvgpu_get_community_stats.argtypes = [vp, vp, vp, vp]
+        L.mvgpu_get_compact_communities.argtypes = [vp, vp]
         L.mvgpu_upload_shard32.argtypes = [vp, ctypes.c_int32, vp, ctypes.c_int32, ctypes.c_int32, vp, vp]
         L.mvgpu_louvain32.argtypes = [vp, ctypes.c_float, ctypes.c_float, ctypes.POINTER(ci), ctypes.POINTER(ctypes.c_float)]
         L.mvgpu_get_communities32.argtypes = [vp, vp]
@@ -200,6 +214,39 @@ class LouvainGPU:
         v = ctypes.c_int(0)
         _ck(lib().mvgpu_get_converged(self._h, ctypes.byref(v)))
         return bool(v.value)
+
+    def evaluate(self, comm=None):
+        """Modularity Q and community counts of an assignment (lnv global community ids in [0, nv), caller's vertex
+        numbering, the form set_initial_communities takes); None evaluates what the last louvain() returned.  Collective:
+        every rank passes an array or every rank None; a bad id or an array whose length is not lnv on any rank raises
+        MvgpuError on every rank.  Returns mvgpu_quality as a dict (DESIGN.md §3.10)."""
+        q = Quality()
+        if comm is None:
+            _ck(lib().mvgpu_evaluate_communities(self._h, None, ctypes.byref(q)))
+            return q.as_dict()
+        comm = np.ascontiguousarray(comm, dtype=np.int64)
+        if comm.ndim != 1 or comm.size != self.lnv:
+            # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
+            why = f"assignment has {comm.size} entries, the shard has lnv = {self.lnv}"
+            _ck(lib().mv_evaluate_refused(self._h, why.encode(), ctypes.byref(q)))
+            raise AssertionError("unreachable: a refused evaluation fails")
+        buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
+        _ck(lib().mvgpu_evaluate_communities(self._h, buf.ctypes.data, ctypes.byref(q)))
+        return q.as_dict()
+
+    def community_stats(self):
+        """Per community of the last evaluate(): entry s describes community parts[rank] + s.  Returns a dict of
+        `size` (int64), `volume` and `internal` (float64), lnv entries each."""
+        n = max(self.lnv, 1)
+        size, vol, internal = np.zeros(n, np.int64), np.zeros(n, np.float64), np.zeros(n, np.float64)
+        _ck(lib().mvgpu_get_community_stats(self._h, size.ctypes.data, vol.ctypes.data, internal.ctypes.data))
+        return {"size": size[:self.lnv], "volume": vol[:self.lnv], "internal": internal[:self.lnv]}
+
+    def compact_communities(self):
+        """Per vertex of the last evaluate(): its community's rank among the non-empty ids in ascending id (int64)."""
+        out = np.zeros(max(self.lnv, 1), np.int64)
+        _ck(lib().mvgpu_get_compact_communities(self._h, out.ctypes.data))
+        return out[:self.lnv]
 
     def communities(self, out=None):
         """currComm of this rank's vertices (global community ids).  `out`: optional preallocated int64 array
