@@ -10,7 +10,8 @@
 // (comm_mode 1), as this library's own kernels over the same peer memory: k_push_ghosts stores every send segment
 // straight into the ghost tail of the peer's community array, k_p2p_barrier / k_p2p_allreduce are flag-based
 // collectives.  comm_mode 0 keeps them as one grouped ncclSend/ncclRecv all-to-all-v with run-constant counts plus
-// one ncclAllReduce of two doubles.  The setup exchanges (ghost lists, counts, IPC handles) always use NCCL.
+// one ncclAllReduce of two doubles.  The setup exchanges (ghost lists, counts, IPC handles) go through NCCL, or through
+// the host transport (option host_transport=1, a shared-memory segment) that also lets ranks share one device.
 #include <cuda_runtime.h>
 #include <unistd.h>
 
@@ -23,6 +24,7 @@
 #include <random>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/mvgpu.h"
@@ -84,12 +86,47 @@ struct DevBuf {              // grow-only device buffer (allocations are cached 
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
-constexpr int kPeerArrays = 13;
+// The arrays every rank exports to its peers (CUDA IPC, or plain pointers between threads of one process), listed here
+// only: X(buffer, exported by this run, the size a run ensures it at (0: not allocated by this run), where rank r's
+// copy is bound).  need_v = lnv, need_s = lnv + the non-owned edge tails.
+#define MV_EXPORTS(X)                                               \
+  X(cdeg, c->unit, need_v, c->pt.cdeg[r])                           \
+  X(csize, c->unit, need_v, c->pt.csize[r])                         \
+  X(upd, c->unit, need_v, c->pt.upd[r])                             \
+  X(cinfo_w, !c->unit, need_v, c->pt.cinfo_w[r])                    \
+  X(usize, !c->unit, need_v, c->pt.usize[r])                        \
+  X(udeg, !c->unit, need_v, c->pt.udeg[r])                          \
+  X(lab, c->relabel, need_v, c->pt.lab[r])                          \
+  X(comm_a, true, need_s, c->peer_comm[0][r])                       \
+  X(comm_b, true, need_s, c->peer_comm[1][r])                       \
+  X(p2p, true, 1, c->pp.st[r])                                      \
+  X(inv, c->relabel, need_v, c->peer_inv[r])                        \
+  X(q_internal, true, ev ? need_v : 0, c->qp.internal[r])           \
+  X(q_rank, true, ev ? need_v + 1 : 0, c->qp.rank[r])
+#define MV_COUNT(...) +1
+constexpr int kPeerArrays = 0 MV_EXPORTS(MV_COUNT);
+#undef MV_COUNT
+
+struct Export {
+  void *p;                             // NULL: this run does not export the array
+  unsigned gen;                        // its DevBuf generation
+  size_t cap, need;                    // its capacity (0: not allocated) and the size this run ensures (0: none)
+};
 
 struct PeerBlob {            // what every rank publishes about its community arrays
   cudaIpcMemHandle_t h[kPeerArrays];
   unsigned long long raw[kPeerArrays];
   int pid, device, unit, pad;
+};
+
+// what the last setup decided about the layout, kept on the host for mv_layout_readback (a test hook, not in mvgpu.h);
+// every value is one that setup_run or run_louvain already had on the host
+struct LayoutReport {
+  int want = 0, stride = 0, unordered = 0, has_self = 0;
+  long long nregions = 0;
+  long long span[2] = {-1, -1};       // k_span_sample's sum and count; -1: the sample did not run
+  bool first_ran = false;             // iteration 1 launched k_scan_pw's FIRST instantiation
+  const int32_t *tails = nullptr;     // the compact tails before renumbering (c->tails or the uploaded compact array)
 };
 
 }  // namespace
@@ -140,14 +177,7 @@ struct mvgpu_ctx {
   bool reordered = false;
   int relabel = 0;
   double reorder_s = 0.0;
-  // what the last setup decided, kept on the host for mv_layout_readback (a test hook, not in mvgpu.h); every value is
-  // one that setup_run or run_louvain already had on the host
-  int lay_want = 0, lay_stride = 0;
-  long long lay_nregions = 0;
-  long long lay_span[2] = {-1, -1};   // k_span_sample's sum and count; -1: the sample did not run
-  int lay_unordered = 0, lay_has_self = 0;
-  bool lay_first_ran = false;         // iteration 1 launched k_scan_pw's FIRST instantiation
-  const int32_t *lay_tails = nullptr; // the compact tails before renumbering (c->tails or the uploaded compact array)
+  LayoutReport lay;
   DevBuf<double> self_d, vdeg;
   // state
   DevBuf<int32_t> comm_a, comm_b;
@@ -185,10 +215,8 @@ struct mvgpu_ctx {
   PeerTable pt;
   std::vector<void *> ipc_opened;
   bool peers_ready = false, ipc_valid = false;
-  int peers_unit = -1;
   const int32_t *peer_inv[kMaxRanks];  // every rank's inv (old -> new local index) while some rank renumbers: warm-start init only
-  void *last_ptrs[kPeerArrays] = {};
-  unsigned last_gens[kPeerArrays] = {};
+  Export last_export[kPeerArrays] = {};   // what the last IPC exchange published
   // options
   int opt_trace = 0, opt_force_weighted = 0, opt_scan_variant = 6, opt_cache_policy = 5, opt_reorder = 2, opt_region = 512, opt_comm_mode = 1, opt_compact_upload = 0, opt_host_threads = 8, opt_first_iter = 1, opt_host_transport = 0;
   long long opt_upload_chunk = 4LL << 20;
@@ -257,6 +285,7 @@ struct Scalars {
   unsigned long long span_sum, span_cnt;
   unsigned long long q_agg[2];         // evaluation: singletons, largest community
 };
+Scalars *dev_scalars(mvgpu_ctx *c) { return reinterpret_cast<Scalars *>(c->scratch.p); }
 
 // ---- setup-time collectives (a handful per run): NCCL on the library's stream, or the host transport ----------------
 int coll_sync(mvgpu_ctx *c) { CK(cudaStreamSynchronize(c->stream)); return 0; }
@@ -269,7 +298,7 @@ int coll_allreduce_i64(mvgpu_ctx *c, long long *v, int n, bool is_max) {
     else c->hc.allreduce(v, n, [](long long a, long long b) { return a + b; });
     return 0;
   }
-  long long *d = reinterpret_cast<Scalars *>(c->scratch.p)->counts;
+  long long *d = dev_scalars(c)->counts;
   CK(cudaMemcpyAsync(d, v, sizeof(long long) * n, cudaMemcpyHostToDevice, c->stream));
   NK(g_nccl.AllReduce(d, d, n, ncclInt64, is_max ? ncclMax : ncclSum, c->comm, c->stream));
   CK(cudaMemcpyAsync(v, d, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
@@ -317,7 +346,7 @@ int coll_alltoallv_dev(mvgpu_ctx *c, const void *d_send, const std::vector<long 
 int coll_barrier(mvgpu_ctx *c) {
   if (c->nranks == 1) return coll_sync(c);
   if (c->hc.is_open()) { TRY(coll_sync(c)); c->hc.barrier(); return 0; }
-  long long *d = reinterpret_cast<Scalars *>(c->scratch.p)->counts;
+  long long *d = dev_scalars(c)->counts;
   NK(g_nccl.AllReduce(d, d, 1, ncclInt64, ncclSum, c->comm, c->stream));
   return coll_sync(c);
 }
@@ -338,96 +367,120 @@ int set_graph(mvgpu_ctx *c, long long nv_global, const int64_t *parts, long long
   c->nv_global = nv_global; c->lnv = lnv; c->lne = lne;
   c->have_graph = true;
   c->peers_ready = false;
+  c->d_rowptr64 = nullptr; c->d_edges = nullptr; c->d_tails32 = nullptr;   // set_source names the new shard's arrays
   return 0;
 }
 
-// ---- multi-GPU: publish/obtain peer pointers for the community arrays -------------------------
-int setup_peers(mvgpu_ctx *c, int unit) {
-  PeerTable &pt = c->pt;
-  pt.nranks = c->nranks; pt.rank = c->rank;
-  for (int r = 0; r <= c->nranks; r++) pt.parts[r] = c->parts[r];
-  if (c->nranks == 1) {
-    pt.lab[0] = c->relabel ? c->lab.p : nullptr;
-    pt.cdeg[0] = c->cdeg.p; pt.csize[0] = c->csize.p; pt.upd[0] = c->upd.p; pt.cinfo_w[0] = c->cinfo_w.p; pt.usize[0] = c->usize.p; pt.udeg[0] = c->udeg.p;
-    c->peer_inv[0] = c->relabel ? c->inv.p : nullptr;
-    c->qp.internal[0] = c->q_internal.p; c->qp.rank[0] = c->q_rank.p;
-    return 0;
-  }
-  // the evaluation arrays are exported whenever they exist (an evaluation allocated them), so that alternating runs
-  // and evaluations reopen no mapping for them; lab / inv still differ between a renumbering run (exported) and an
-  // evaluation (never renumbers: NULL), so switching between those two reopens the mappings
-  void *ptrs[kPeerArrays] = {unit ? (void *)c->cdeg.p : nullptr, unit ? (void *)c->csize.p : nullptr, unit ? (void *)c->upd.p : nullptr,
-                    unit ? nullptr : (void *)c->cinfo_w.p, unit ? nullptr : (void *)c->usize.p,
-                    unit ? nullptr : (void *)c->udeg.p, c->relabel ? (void *)c->lab.p : nullptr,
-                    (void *)c->comm_a.p, (void *)c->comm_b.p, (void *)c->p2p.p, c->relabel ? (void *)c->inv.p : nullptr,
-                    (void *)c->q_internal.p, (void *)c->q_rank.p};
-  if (c->peers_ready) return 0;            // same graph, same buffers: tables are still valid
-  // IPC handles are expensive to (re)open: skip the exchange when no rank's buffers moved since the last one
-  const unsigned gens[kPeerArrays] = {c->cdeg.gen, c->csize.gen, c->upd.gen, c->cinfo_w.gen, c->usize.gen, c->udeg.gen, c->lab.gen,
-                                      c->comm_a.gen, c->comm_b.gen, c->p2p.gen, c->inv.gen, c->q_internal.gen, c->q_rank.gen};
-  long long changed = c->ipc_valid ? 0 : 1;
-  for (int k = 0; k < kPeerArrays; k++) if (ptrs[k] != c->last_ptrs[k] || (ptrs[k] && gens[k] != c->last_gens[k])) changed = 1;
-  TRY(coll_allreduce_i64(c, &changed, 1, true));
-  if (changed) {
+// where setup_run reads the shard set_graph described (full records or compact tails) and what uploading it cost
+void set_source(mvgpu_ctx *c, const long long *rowptr64, const Edge16 *edges, const int32_t *tails32, bool f32, double h2d_s,
+                long long h2d_bytes) {
+  c->d_rowptr64 = rowptr64; c->d_edges = edges; c->d_tails32 = tails32; c->f32 = f32;
+  c->h2d_s = h2d_s; c->h2d_bytes = h2d_bytes;
+}
+
+// CUB's two-phase protocol for one or more calls that share c->cub_tmp: every size query, one (grow-only) ensure of the
+// largest, then the calls in order.  Each f(temp, bytes) is one CUB call.
+template <typename... F>
+int cub_run(mvgpu_ctx *c, F &&...f) {
+  size_t need = 0;
+  auto query = [&](auto &g) { size_t tb = 0; g(nullptr, tb); need = std::max(need, tb); };
+  (query(f), ...);
+  TRY(c->cub_tmp.ensure(need));
+  cudaError_t e = cudaSuccess;
+  auto call = [&](auto &g) { size_t tb = c->cub_tmp.cap; if (e == cudaSuccess) e = g(c->cub_tmp.p, tb); };
+  (call(f), ...);
+  CK(e);
+  return 0;
+}
+
+// ---- multi-GPU: publish/obtain peer pointers for the exported arrays (MV_EXPORTS) ------------------------------------
+// this rank's exported arrays, in MV_EXPORTS order (the sizes matter to the grow test of setup_agree only)
+void exports(const mvgpu_ctx *c, Export (&x)[kPeerArrays], size_t need_v = 0, size_t need_s = 0, bool ev = false) {
+  int k = 0;
+#define MV_EXPORT(buf, on, need, dst) x[k++] = {(on) ? (void *)c->buf.p : nullptr, c->buf.gen, c->buf.cap, (size_t)(need)};
+  MV_EXPORTS(MV_EXPORT)
+#undef MV_EXPORT
+}
+
+// rank r's copies of the exported arrays (q in MV_EXPORTS order) -> the peer tables
+void bind_peer(mvgpu_ctx *c, int r, void *const *q) {
+  int k = 0;
+#define MV_BIND(buf, on, need, dst) dst = static_cast<std::remove_reference_t<decltype(dst)>>(q[k++]);
+  MV_EXPORTS(MV_BIND)
+#undef MV_BIND
+}
+
+void close_ipc(mvgpu_ctx *c) {
   for (void *p : c->ipc_opened) cudaIpcCloseMemHandle(p);
   c->ipc_opened.clear();
   c->ipc_valid = false;
-  PeerBlob mine;
-  memset(&mine, 0, sizeof mine);
-  for (int k = 0; k < kPeerArrays; k++) {
-    mine.raw[k] = (unsigned long long)ptrs[k];
-    if (ptrs[k]) CK(cudaIpcGetMemHandle(&mine.h[k], ptrs[k]));
-  }
-  mine.pid = (int)getpid(); mine.device = c->device; mine.unit = unit;
-  std::vector<PeerBlob> all(c->nranks);
-  TRY(coll_allgather(c, &mine, all.data(), sizeof(PeerBlob)));
-  for (int r = 0; r < c->nranks; r++) {
-    void *q[kPeerArrays] = {};
-    if (all[r].unit != unit) return fail("ranks disagree on the unit-weight path");
-    if (r == c->rank) { for (int k = 0; k < kPeerArrays; k++) q[k] = ptrs[k]; }
-    else if (all[r].pid == mine.pid) {           // same process (threads): plain UVA pointers + peer access
-      if (all[r].device != c->device) {          // ranks sharing one device need no peer mapping at all
-        int can = 0;
-        CK(cudaDeviceCanAccessPeer(&can, c->device, all[r].device));
-        if (!can) return fail("GPU " + std::to_string(c->device) + " cannot access peer GPU " + std::to_string(all[r].device));
-        cudaError_t e = cudaDeviceEnablePeerAccess(all[r].device, 0);
-        if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CK(e);
-        cudaGetLastError();
-      }
-      for (int k = 0; k < kPeerArrays; k++) q[k] = (void *)all[r].raw[k];
-    } else {
-      for (int k = 0; k < kPeerArrays; k++)
-        if (all[r].raw[k]) {
-          CK(cudaIpcOpenMemHandle(&q[k], all[r].h[k], cudaIpcMemLazyEnablePeerAccess));
-          c->ipc_opened.push_back(q[k]);
-        }
+}
+
+int setup_peers(mvgpu_ctx *c) {
+  PeerTable &pt = c->pt;
+  pt.nranks = c->nranks; pt.rank = c->rank;
+  for (int r = 0; r <= c->nranks; r++) pt.parts[r] = c->parts[r];
+  Export x[kPeerArrays];
+  exports(c, x);
+  void *ptrs[kPeerArrays];
+  for (int k = 0; k < kPeerArrays; k++) ptrs[k] = x[k].p;
+  if (c->nranks == 1) { bind_peer(c, 0, ptrs); return 0; }
+  if (c->peers_ready) return 0;            // same graph, same buffers: tables are still valid
+  // IPC handles are expensive to (re)open: skip the exchange when no rank's buffers moved since the last one.  The
+  // evaluation arrays are exported whenever they exist, so alternating runs and evaluations reopen no mapping for them;
+  // lab / inv are exported by a renumbering run and never by an evaluation, so switching between those two does.
+  long long changed = c->ipc_valid ? 0 : 1;
+  for (int k = 0; k < kPeerArrays; k++) if (ptrs[k] != c->last_export[k].p || (ptrs[k] && x[k].gen != c->last_export[k].gen)) changed = 1;
+  TRY(coll_allreduce_i64(c, &changed, 1, true));
+  if (changed) {
+    close_ipc(c);
+    PeerBlob mine;
+    memset(&mine, 0, sizeof mine);
+    for (int k = 0; k < kPeerArrays; k++) {
+      mine.raw[k] = (unsigned long long)ptrs[k];
+      if (ptrs[k]) CK(cudaIpcGetMemHandle(&mine.h[k], ptrs[k]));
     }
-    pt.cdeg[r] = (const uint32_t *)q[0]; pt.csize[r] = (const int32_t *)q[1]; pt.upd[r] = (unsigned long long *)q[2];
-    pt.cinfo_w[r] = (const CommW *)q[3]; pt.usize[r] = (long long *)q[4]; pt.udeg[r] = (double *)q[5];
-    pt.lab[r] = (const int32_t *)q[6];
-    c->peer_comm[0][r] = (int32_t *)q[7]; c->peer_comm[1][r] = (int32_t *)q[8];
-    c->pp.st[r] = (P2PState *)q[9];
-    c->peer_inv[r] = (const int32_t *)q[10];
-    c->qp.internal[r] = (double *)q[11]; c->qp.rank[r] = (const int32_t *)q[12];
-  }
-  for (int k = 0; k < kPeerArrays; k++) { c->last_ptrs[k] = ptrs[k]; c->last_gens[k] = gens[k]; }
-  c->ipc_valid = true;
+    mine.pid = (int)getpid(); mine.device = c->device; mine.unit = c->unit ? 1 : 0;
+    std::vector<PeerBlob> all(c->nranks);
+    TRY(coll_allgather(c, &mine, all.data(), sizeof(PeerBlob)));
+    for (int r = 0; r < c->nranks; r++) {
+      void *q[kPeerArrays] = {};
+      if (all[r].unit != mine.unit) return fail("ranks disagree on the unit-weight path");
+      if (r == c->rank) { for (int k = 0; k < kPeerArrays; k++) q[k] = ptrs[k]; }
+      else if (all[r].pid == mine.pid) {           // same process (threads): plain UVA pointers + peer access
+        if (all[r].device != c->device) {          // ranks sharing one device need no peer mapping at all
+          int can = 0;
+          CK(cudaDeviceCanAccessPeer(&can, c->device, all[r].device));
+          if (!can) return fail("GPU " + std::to_string(c->device) + " cannot access peer GPU " + std::to_string(all[r].device));
+          cudaError_t e = cudaDeviceEnablePeerAccess(all[r].device, 0);
+          if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CK(e);
+          cudaGetLastError();
+        }
+        for (int k = 0; k < kPeerArrays; k++) q[k] = (void *)all[r].raw[k];
+      } else {
+        for (int k = 0; k < kPeerArrays; k++)
+          if (all[r].raw[k]) {
+            CK(cudaIpcOpenMemHandle(&q[k], all[r].h[k], cudaIpcMemLazyEnablePeerAccess));
+            c->ipc_opened.push_back(q[k]);
+          }
+      }
+      bind_peer(c, r, q);
+    }
+    std::copy(x, x + kPeerArrays, c->last_export);
+    c->ipc_valid = true;
   }
   // where my send segments land in each peer's community array: its lnv + its receive offset for me
-  {
-    std::vector<long long> gb(c->nranks), allgb((size_t)c->nranks * c->nranks);
-    for (int r = 0; r < c->nranks; r++) gb[r] = c->lnv + c->roff[r];
-    TRY(coll_allgather(c, gb.data(), allgb.data(), sizeof(long long) * c->nranks));
-    for (int b = 0; b < 2; b++) {
-      PushTable &t = c->push[b];
-      t.nranks = c->nranks;
-      for (int r = 0; r <= c->nranks; r++) t.soff[r] = c->soff[r];
-      for (int r = 0; r < c->nranks; r++) t.dst[r] = c->peer_comm[b][r] + allgb[(size_t)r * c->nranks + c->rank];
-    }
-    c->pp.rank = c->rank; c->pp.nranks = c->nranks;
+  std::vector<long long> gb(c->nranks), allgb((size_t)c->nranks * c->nranks);
+  for (int r = 0; r < c->nranks; r++) gb[r] = c->lnv + c->roff[r];
+  TRY(coll_allgather(c, gb.data(), allgb.data(), sizeof(long long) * c->nranks));
+  for (int b = 0; b < 2; b++) {
+    PushTable &t = c->push[b];
+    t.nranks = c->nranks;
+    for (int r = 0; r <= c->nranks; r++) t.soff[r] = c->soff[r];
+    for (int r = 0; r < c->nranks; r++) t.dst[r] = c->peer_comm[b][r] + allgb[(size_t)r * c->nranks + c->rank];
   }
+  c->pp.rank = c->rank; c->pp.nranks = c->nranks;
   c->peers_ready = true;
-  c->peers_unit = unit * 2 + c->relabel;
   return 0;
 }
 
@@ -466,7 +519,7 @@ int launch_scan_t(mvgpu_ctx *c, const ScanParams &sp, bool first) {
     const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, pw_ctas_per_sm * c->num_sms);
     if (UNIT && first) {
       k_scan_pw<UNIT, MULTI, TRACE, UNIT><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
-      c->lay_first_ran = true;
+      c->lay.first_ran = true;
     } else k_scan_pw<UNIT, MULTI, TRACE, false><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
     c->tm.kernel_launches++; c->tm.scan_launches++;
   } else if (tiles > 0) {
@@ -540,23 +593,17 @@ struct EvalSetup {
   std::string err;
 };
 
-// ---- setup: reference-format arrays -> compact graph, ghosts, init ------------------------------
-// ev != nullptr: setup for an evaluation -- warm init from ev->X, no locality renumbering, evaluation arrays allocated
-int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
-  cudaStream_t s = c->stream;
-  const int nsm = c->num_sms;
-  TRY(c->scratch.ensure(sizeof(Scalars)));
-  Scalars *d_sc = reinterpret_cast<Scalars *>(c->scratch.p);
-  Scalars h;
-  CK(cudaMemsetAsync(d_sc, 0, sizeof(Scalars), s));
-  const long long lnv = c->lnv, lne = c->lne;
-  c->warm_run = ev ? true : c->have_init;
+// the compact CSR the iterations run on: the converted shard, then possibly its renumbered copy
+struct Csr { const uint32_t *rowptr = nullptr; const int32_t *tails = nullptr; const double *weights = nullptr; };
 
-  // pass 1 over the edges: unit weights? how many non-owned tails? (+ input validation).  The compact upload
-  // format has answered all of that on the host already.
+// ---- setup: reference-format arrays -> compact graph, ghosts, init, as the stages of setup_run ------------------------
+// Pass 1 over the edges: unit weights? how many non-owned tails? (+ input validation).  The compact upload format has
+// answered all of that on the host already.  h: the device scalars after the pass; err: what this rank finds wrong.
+int input_pass(mvgpu_ctx *c, const EvalSetup *ev, Scalars &h, int &unit, std::string &err) {
+  cudaStream_t s = c->stream; const int nsm = c->num_sms; Scalars *d_sc = dev_scalars(c);
+  const long long lnv = c->lnv, lne = c->lne;
   const bool compact_in = c->d_tails32 != nullptr;
-  const bool fused_stats = !compact_in && c->nranks == 1;      // single rank: statistics ride on the conversion pass
-  if (fused_stats) {
+  if (!compact_in && c->nranks == 1) {      // single rank: statistics ride on the conversion pass
     TRY(c->tails.ensure(lne + 4));
     k_convert_edges<<<grid_for(lne, 256, nsm, 16), 256, 0, s>>>(c->d_edges, lne, c->base, c->bound, c->nv_global, c->tails.p,
                                                               nullptr, nullptr, nullptr, nullptr, &d_sc->st);
@@ -571,71 +618,71 @@ int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
   CK(cudaMemcpyAsync(&h, d_sc, sizeof h, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (compact_in) { h.st.nremote = (unsigned long long)c->in_nremote; h.st.nonunit = 0; h.st.bad_tail = 0; }
-  // input errors are agreed on across ranks before anybody returns: a rank that left alone would leave its peers
-  // blocked in the next collective
-  std::string input_err;
-  if (h.st.bad_tail) input_err = "edge tail outside [0, nv)";
-  else if (h.bad_rowptr) input_err = "edge_indices malformed (must start at 0, end at lne and never decrease)";
-  else if (c->nranks == 1 && h.st.nremote) input_err = "non-local tail in a single-rank graph";
+  if (h.st.bad_tail) err = "edge tail outside [0, nv)";
+  else if (h.bad_rowptr) err = "edge_indices malformed (must start at 0, end at lne and never decrease)";
+  else if (c->nranks == 1 && h.st.nremote) err = "non-local tail in a single-rank graph";
   c->maxdeg = h.maxdeg;
-  int unit = (!h.st.nonunit && !c->opt_force_weighted) ? 1 : 0;
-  if (input_err.empty() && compact_in && !unit) input_err = "force_weighted needs the full edge records: set compact_upload=0";
-  if (input_err.empty() && ev) input_err = ev->err;
+  unit = (!h.st.nonunit && !c->opt_force_weighted) ? 1 : 0;
+  if (err.empty() && compact_in && !unit) err = "force_weighted needs the full edge records: set compact_upload=0";
+  if (err.empty() && ev) err = ev->err;
+  return 0;
+}
 
-  // global agreement on the path + on 2m < 2^31 needs the total weight; the weight total itself comes
-  // from the vertex-init kernel below, so first settle `unit` from the flags (ne bound checked after).
-  long long ne_global = lne;
+// The one setup agreement (one all-reduce): path, edge total, input errors, "must grow an exported array", "was given
+// an assignment".  Errors are agreed on before anybody returns: a rank that left alone would leave its peers blocked in
+// the next collective.  Sets c->unit (2m < 2^31 settles from the edge total; the weight total comes later).
+int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, std::string err) {
+  long long ne_global = c->lne;
   if (c->nranks > 1) {
-    // exported (peer-mapped) arrays that this run may have to grow: CUDA IPC requires every peer to close its
-    // mapping before the owner frees the block, so that is agreed on here and done collectively
-    const size_t need_v = (size_t)lnv, need_s = (size_t)(lnv + (long long)h.st.nremote);
-    const bool grow = c->ipc_valid && ((c->cdeg.p && c->cdeg.cap < need_v) || (c->cinfo_w.p && c->cinfo_w.cap < need_v) ||
-                                       (c->lab.p && c->lab.cap < need_v) || (c->inv.p && c->inv.cap < need_v) ||
-                                       c->comm_a.cap < need_s || c->comm_b.cap < need_s ||
-                                       (ev && ((c->q_internal.p && c->q_internal.cap < need_v) ||
-                                               (c->q_rank.p && c->q_rank.cap < need_v + 1))));
+    // CUDA IPC requires every peer to close its mapping before the owner frees the block, so growing an exported array
+    // is agreed on here and done collectively (need_s: init_state's bound lnv + #non-owned edge tails >= lnv + nghost)
+    Export x[kPeerArrays];
+    exports(c, x, (size_t)c->lnv, (size_t)(c->lnv + nremote), ev != nullptr);
+    bool grow = false;
+    for (const Export &e : x) grow = grow || (c->ipc_valid && e.cap && e.cap < e.need);
     const bool assigned = ev ? ev->given : c->warm_run;
-    long long hv[5] = {unit ? 0 : 1, lne, input_err.empty() ? 0 : 1, grow ? 1 : 0, assigned ? 1 : 0};
+    long long hv[5] = {unit ? 0 : 1, c->lne, err.empty() ? 0 : 1, grow ? 1 : 0, assigned ? 1 : 0};
     TRY(coll_allreduce_i64(c, hv, 5, false));
     unit = hv[0] == 0;
     ne_global = hv[1];
-    if (hv[2] && input_err.empty()) input_err = ev ? "another rank rejected its shard or its assignment" : "another rank rejected its shard";
-    if (input_err.empty() && hv[4] != 0 && hv[4] != c->nranks)
-      input_err = ev ? "ranks disagree on the assignment to evaluate: every rank or none must pass NULL"
-                     : "ranks disagree on the initial assignment: every rank or none must set one";
+    if (hv[2] && err.empty()) err = ev ? "another rank rejected its shard or its assignment" : "another rank rejected its shard";
+    if (err.empty() && hv[4] != 0 && hv[4] != c->nranks)
+      err = ev ? "ranks disagree on the assignment to evaluate: every rank or none must pass NULL"
+               : "ranks disagree on the initial assignment: every rank or none must set one";
     if (hv[3]) {
-      for (void *q : c->ipc_opened) cudaIpcCloseMemHandle(q);
-      c->ipc_opened.clear();
-      c->ipc_valid = false;
+      close_ipc(c);
       c->peers_ready = false;
       TRY(coll_barrier(c));                       // all mappings are closed before any owner reallocates
     }
   }
-  if (!input_err.empty()) return fail(input_err);
+  if (!err.empty()) return fail(err);
   if (unit && ne_global >= (1LL << 31)) unit = 0;   // packed 32-bit degree deltas need 2m < 2^31
   c->unit = unit != 0;
+  return 0;
+}
 
-  // pass 2: tails -> slots, weights split off, remote tails listed
-  const long long nremote = (long long)h.st.nremote;
+// pass 2: tails -> slots, weights split off, remote tails listed
+int compact_edges(mvgpu_ctx *c, long long nremote, Csr &g) {
+  cudaStream_t s = c->stream; const int nsm = c->num_sms; Scalars *d_sc = dev_scalars(c);
+  const long long lne = c->lne;
+  const bool compact_in = c->d_tails32 != nullptr;
   if (nremote) { TRY(c->remote_list.ensure(nremote)); TRY(c->remote_pos.ensure(nremote)); }
-  const uint32_t *src_rowptr = c->rowptr.p;
-  const int32_t *src_tails = nullptr;
-  const double *src_weights = nullptr;
+  g.rowptr = c->rowptr.p;
   if (compact_in && c->nranks == 1) {
-    src_tails = c->d_tails32;                       // global id == local slot: the uploaded array is used as is (read-only)
-    if (!c->unit) {                                 // 2m >= 2^31: fp64 path on a shard that arrived without weights
+    g.tails = c->d_tails32;                       // global id == local slot: the uploaded array is used as is (read-only)
+    if (!c->unit) {                               // 2m >= 2^31: fp64 path on a shard that arrived without weights
       TRY(c->weights.ensure(lne + 4));
       k_fill_ones<<<grid_for(lne, 256, nsm, 16), 256, 0, s>>>(c->weights.p, lne);
       c->tm.kernel_launches++;
-      src_weights = c->weights.p;
+      g.weights = c->weights.p;
     }
-  } else if (fused_stats) {
-    src_tails = c->tails.p;                         // converted by the fused pass above
+  } else if (c->nranks == 1) {
+    g.tails = c->tails.p;                         // converted by input_pass
     if (!c->unit) {
       TRY(c->weights.ensure(lne + 4));
       k_extract_weights<<<grid_for(lne, 256, nsm, 16), 256, 0, s>>>(c->d_edges, lne, c->weights.p);
       c->tm.kernel_launches++;
-      src_weights = c->weights.p;
+      g.weights = c->weights.p;
     }
   } else {
     TRY(c->tails.ensure(lne + 4));
@@ -648,181 +695,173 @@ int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
                                                                 c->unit ? nullptr : c->weights.p,
                                                                 nremote ? c->remote_list.p : nullptr, c->remote_pos.p, &d_sc->remote_cursor, nullptr);
     c->tm.kernel_launches++;
-    if (compact_in && !c->unit) {                   // a peer's shard is weighted (or 2m >= 2^31): this one's weights are all 1.0
+    if (compact_in && !c->unit) {                 // a peer's shard is weighted (or 2m >= 2^31): this one's weights are all 1.0
       k_fill_ones<<<grid_for(lne, 256, nsm, 16), 256, 0, s>>>(c->weights.p, lne);
       c->tm.kernel_launches++;
     }
-    src_tails = c->tails.p;
-    src_weights = c->unit ? nullptr : c->weights.p;
+    g.tails = c->tails.p;
+    g.weights = c->unit ? nullptr : c->weights.p;
   }
+  return 0;
+}
 
-  // ghost discovery (exchangeVertexReqs, dspl.hpp:1106-1272): sorted unique non-owned tails
+// ghost discovery (exchangeVertexReqs, dspl.hpp:1106-1272): sorted unique non-owned tails, per-peer counts both ways,
+// and the send lists
+int discover_ghosts(mvgpu_ctx *c, long long nremote) {
+  cudaStream_t s = c->stream; const int nsm = c->num_sms; Scalars *d_sc = dev_scalars(c);
+  const long long lnv = c->lnv;
   c->nghost = 0; c->nsend = 0;
   c->rcount.assign(c->nranks, 0); c->scount.assign(c->nranks, 0);
   c->roff.assign(c->nranks + 1, 0); c->soff.assign(c->nranks + 1, 0);
-  if (c->nranks > 1) {
-    if (nremote) {
-      DevBuf<long long> &sorted = c->sorted_tmp;   // grow-only: no cudaMalloc/cudaFree inside the timed setup after the first run
-      TRY(sorted.ensure(nremote));
-      TRY(c->ghost_gid.ensure(nremote));
-      size_t tb1 = 0, tb2 = 0;
-      int bits = 1;
-      while ((1LL << bits) < c->nv_global && bits < 63) bits++;
-      cub::DeviceRadixSort::SortKeys(nullptr, tb1, c->remote_list.p, sorted.p, nremote, 0, bits, s);
-      cub::DeviceSelect::Unique(nullptr, tb2, sorted.p, c->ghost_gid.p, &d_sc->nunique, nremote, s);
-      TRY(c->cub_tmp.ensure(std::max(tb1, tb2)));
-      size_t tb = c->cub_tmp.cap;
-      CK(cub::DeviceRadixSort::SortKeys(c->cub_tmp.p, tb, c->remote_list.p, sorted.p, nremote, 0, bits, s));
-      tb = c->cub_tmp.cap;
-      CK(cub::DeviceSelect::Unique(c->cub_tmp.p, tb, sorted.p, c->ghost_gid.p, &d_sc->nunique, nremote, s));
-      c->tm.kernel_launches += 2;
-      int nu = 0;
-      CK(cudaMemcpyAsync(&nu, &d_sc->nunique, sizeof nu, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      c->nghost = nu;
-      if (lnv + c->nghost >= (1LL << 31)) return fail("lnv + nghost >= 2^31");
-      k_remap_ghost_tails<<<grid_for(nremote, 256, nsm, 16), 256, 0, s>>>(c->remote_list.p, c->remote_pos.p, nremote, c->tails.p, c->ghost_gid.p, (int)c->nghost, (int)lnv);
-      c->tm.kernel_launches++;
-      // per-owner counts of my ghosts (the list is sorted, owners are contiguous ranges)
-      std::vector<long long> hg(c->nghost);
-      CK(cudaMemcpyAsync(hg.data(), c->ghost_gid.p, sizeof(long long) * c->nghost, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      for (int r = 0; r < c->nranks; r++) {
-        const long long lo = std::lower_bound(hg.begin(), hg.end(), c->parts[r]) - hg.begin();
-        const long long hi = std::lower_bound(hg.begin(), hg.end(), c->parts[r + 1]) - hg.begin();
-        c->rcount[r] = hi - lo;
-      }
-    }
-    for (int r = 0; r < c->nranks; r++) c->roff[r + 1] = c->roff[r] + c->rcount[r];
-    // tell every owner how many of its vertices I ghost (MPI_Alltoall of sizes, dspl.hpp:1184)
-    {
-      std::vector<long long> allc((size_t)c->nranks * c->nranks);
-      TRY(coll_allgather(c, c->rcount.data(), allc.data(), sizeof(long long) * c->nranks));
-      for (int r = 0; r < c->nranks; r++) c->scount[r] = allc[(size_t)r * c->nranks + c->rank];
-    }
-    for (int r = 0; r < c->nranks; r++) c->soff[r + 1] = c->soff[r] + c->scount[r];
-    c->nsend = c->soff[c->nranks];
-    // ship the ghost id lists to their owners (dspl.hpp:1228-1252); they become the owners' send lists
-    TRY(c->send_gid.ensure(c->nsend));
-    TRY(c->send_lid.ensure(c->nsend));
-    TRY(c->send_buf.ensure(c->nsend));
-    TRY(c->ghost_gid.ensure(c->nghost));
-    TRY(coll_alltoallv_dev(c, c->ghost_gid.p, c->rcount, c->roff, c->send_gid.p, c->scount, c->soff, sizeof(long long)));
-    if (c->nsend) {
-      k_gid_to_lid<<<grid_for(c->nsend, 256, nsm), 256, 0, s>>>(c->send_gid.p, (int)c->nsend, c->base, c->send_lid.p);
-      c->tm.kernel_launches++;
+  if (c->nranks == 1) return 0;
+  if (nremote) {
+    DevBuf<long long> &sorted = c->sorted_tmp;   // grow-only: no cudaMalloc/cudaFree inside the timed setup after the first run
+    TRY(sorted.ensure(nremote));
+    TRY(c->ghost_gid.ensure(nremote));
+    int bits = 1;
+    while ((1LL << bits) < c->nv_global && bits < 63) bits++;
+    TRY(cub_run(c,
+                [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortKeys(t, tb, c->remote_list.p, sorted.p, nremote, 0, bits, s); },
+                [&](void *t, size_t &tb) { return cub::DeviceSelect::Unique(t, tb, sorted.p, c->ghost_gid.p, &d_sc->nunique, nremote, s); }));
+    c->tm.kernel_launches += 2;
+    int nu = 0;
+    CK(cudaMemcpyAsync(&nu, &d_sc->nunique, sizeof nu, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    c->nghost = nu;
+    if (lnv + c->nghost >= (1LL << 31)) return fail("lnv + nghost >= 2^31");
+    k_remap_ghost_tails<<<grid_for(nremote, 256, nsm, 16), 256, 0, s>>>(c->remote_list.p, c->remote_pos.p, nremote, c->tails.p, c->ghost_gid.p, (int)c->nghost, (int)lnv);
+    c->tm.kernel_launches++;
+    // per-owner counts of my ghosts (the list is sorted, owners are contiguous ranges)
+    std::vector<long long> hg(c->nghost);
+    CK(cudaMemcpyAsync(hg.data(), c->ghost_gid.p, sizeof(long long) * c->nghost, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (int r = 0; r < c->nranks; r++) {
+      const long long lo = std::lower_bound(hg.begin(), hg.end(), c->parts[r]) - hg.begin();
+      const long long hi = std::lower_bound(hg.begin(), hg.end(), c->parts[r + 1]) - hg.begin();
+      c->rcount[r] = hi - lo;
     }
   }
+  for (int r = 0; r < c->nranks; r++) c->roff[r + 1] = c->roff[r] + c->rcount[r];
+  // tell every owner how many of its vertices I ghost (MPI_Alltoall of sizes, dspl.hpp:1184)
+  std::vector<long long> allc((size_t)c->nranks * c->nranks);
+  TRY(coll_allgather(c, c->rcount.data(), allc.data(), sizeof(long long) * c->nranks));
+  for (int r = 0; r < c->nranks; r++) c->scount[r] = allc[(size_t)r * c->nranks + c->rank];
+  for (int r = 0; r < c->nranks; r++) c->soff[r + 1] = c->soff[r] + c->scount[r];
+  c->nsend = c->soff[c->nranks];
+  // ship the ghost id lists to their owners (dspl.hpp:1228-1252); they become the owners' send lists
+  TRY(c->send_gid.ensure(c->nsend));
+  TRY(c->send_lid.ensure(c->nsend));
+  TRY(c->send_buf.ensure(c->nsend));
+  TRY(c->ghost_gid.ensure(c->nghost));
+  TRY(coll_alltoallv_dev(c, c->ghost_gid.p, c->rcount, c->roff, c->send_gid.p, c->scount, c->soff, sizeof(long long)));
+  if (c->nsend) {
+    k_gid_to_lid<<<grid_for(c->nsend, 256, nsm), 256, 0, s>>>(c->send_gid.p, (int)c->nsend, c->base, c->send_lid.p);
+    c->tm.kernel_launches++;
+  }
+  return 0;
+}
 
-  // ---- locality renumbering (see kernels.cuh): decide, then BFS regions -> sort -> permute the compact CSR
+// locality renumbering (see kernels.cuh): decide, then BFS regions -> sort -> permute the compact CSR g in place of the
+// original numbering; fills c->lay.  An evaluation makes one pass over the edges, which does not pay for a renumbering.
+int renumber(mvgpu_ctx *c, const EvalSetup *ev, Csr &g) {
+  cudaStream_t s = c->stream; const int nsm = c->num_sms; Scalars *d_sc = dev_scalars(c);
+  const long long lnv = c->lnv, lne = c->lne;
   c->reordered = false;
   c->relabel = 0;
-  c->lay_tails = src_tails;
-  c->lay_span[0] = c->lay_span[1] = -1;
-  c->lay_nregions = 0;
-  c->lay_first_ran = false;
-  {
-    // (an evaluation makes one pass over the edges, which does not pay for a renumbering)
-    int want = !ev && c->opt_reorder == 1 ? 1 : 0;
-    if (!ev && c->opt_reorder == 2 && lnv >= 65536) {
-      // auto: renumber when the given numbering has no locality (mean |tail - v| above lnv/64 on a vertex sample)
-      k_span_sample<<<grid_for(lnv / 64 + 1, 256, nsm), 256, 0, s>>>((int)lnv, src_rowptr, src_tails, 64, &d_sc->span_sum, &d_sc->span_cnt);
-      c->tm.kernel_launches++;
-      unsigned long long sp2[2];
-      CK(cudaMemcpyAsync(sp2, &d_sc->span_sum, sizeof sp2, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      if (sp2[1] > 0 && (double)sp2[0] / (double)sp2[1] > (double)lnv / 64.0) want = 1;
-      c->lay_span[0] = (long long)sp2[0]; c->lay_span[1] = (long long)sp2[1];
-    }
-    // region ids have kBfsRegionBits bits: past 2^22 - 1 regions they would spill into the level field (and region
-    // 2^22 - 1 at level 1023 would read as kBfsUnreached), so very large shards get proportionally larger regions
-    const int stride = (int)std::max<long long>(c->opt_region, (lnv + kBfsMaxRegions - 1) / kBfsMaxRegions);
-    c->lay_want = want;
-    c->lay_stride = stride;
-    int any = want;
-    if (c->nranks > 1) {
-      long long hv = want;
-      TRY(coll_allreduce_i64(c, &hv, 1, true));
-      any = hv != 0;
-    }
-    c->relabel = any;                       // labels are needed everywhere as soon as one rank renumbers
-    if (any && lnv > 0) {
-      cudaEvent_t r0 = get_event(c, 2), r1 = get_event(c, 3);
-      CK(cudaEventRecord(r0, s));
-      TRY(c->perm.ensure(lnv)); TRY(c->inv.ensure(lnv)); TRY(c->lab.ensure(lnv)); TRY(c->ids.ensure(lnv));
-      TRY(c->bfs_key.ensure(lnv)); TRY(c->sortkey.ensure(lnv)); TRY(c->sortkey2.ensure(std::max(lnv, 4 * ((lnv + 31) / 32))));
-      TRY(c->deg_new.ensure(lnv + 1)); TRY(c->rowptr2.ensure(lnv + 1 + 40)); TRY(c->tails2.ensure(lne + 4));
-      if (!c->unit) TRY(c->weights2.ensure(lne + 4));
-      const int max_levels = 1023;
-      if (want) {
-        TRY(c->bfs_level_count.ensure(max_levels));
-        int occ = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_msbfs, 256, 0));
-        if (occ < 1) return fail("k_msbfs cannot be made resident");
-        int ilnv = (int)lnv, st = stride, ml = max_levels;
-        const uint32_t *rp = src_rowptr; const int32_t *tl = src_tails; uint32_t *key = c->bfs_key.p;
-        // the BFS queue and its level bitmaps (4 bits per vertex) live in ids and sortkey2, which k_bfs_sortkeys and the
-        // sort only write after the BFS
-        int32_t *q = c->ids.p; unsigned int *lc = c->bfs_level_count.p; uint32_t *lm = c->sortkey2.p;
-        void *args[] = {&ilnv, &rp, &tl, &key, &st, &ml, &q, &lc, &lm};
-        CK(cudaLaunchCooperativeKernel((void *)k_msbfs, dim3(occ * nsm), dim3(256), args, 0, s));
-        // sort by (region, level): only the bits that can be set take part (one radix pass less than a 32-bit sort)
-        const long long nregions = (lnv + stride - 1) / stride;
-        c->lay_nregions = nregions;
-        int sort_bits = (int)kBfsLevelBits;
-        while ((1LL << (sort_bits - (int)kBfsLevelBits)) <= nregions && sort_bits < 32) sort_bits++;
-        const unsigned int unreached_key = sort_bits >= 32 ? 0xFFFFFFFFu : ((1u << sort_bits) - 1u);
-        k_bfs_sortkeys<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->bfs_key.p, c->sortkey.p, c->ids.p, unreached_key);
-        size_t tb = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tb, c->sortkey.p, c->sortkey2.p, c->ids.p, c->perm.p, (int)lnv, 0, sort_bits, s);
-        TRY(c->cub_tmp.ensure(tb));
-        tb = c->cub_tmp.cap;
-        CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tb, c->sortkey.p, c->sortkey2.p, c->ids.p, c->perm.p, (int)lnv, 0, sort_bits, s));
-        c->tm.kernel_launches += 3;
-      } else {
-        // another rank renumbers, this one keeps its order: identity permutation, labels still required
-        k_bfs_sortkeys<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->bfs_key.p, c->sortkey.p, c->perm.p, 0xFFFFFFFFu);
-        c->tm.kernel_launches++;
-      }
-      k_perm_inverse<<<grid_for(lnv + 1, 256, nsm), 256, 0, s>>>((int)lnv, c->perm.p, c->base, want ? nullptr : c->inv.p, c->lab.p, src_rowptr, c->deg_new.p);
-      c->tm.kernel_launches++;
-      if (want) {
-        // inv[old] = new as a second radix sort (keys perm, values the ids 0..lnv-1 still in c->ids): lnv random 4-byte
-        // stores inv[perm[i]] = i cost more than twice as much as the sort's bucketed scatters (DESIGN.md §3.3)
-        int bits = 1;
-        while ((1LL << bits) < lnv && bits < 31) bits++;
-        const uint32_t *pk = reinterpret_cast<const uint32_t *>(c->perm.p);
-        size_t tb = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tb, pk, c->sortkey2.p, c->ids.p, c->inv.p, (int)lnv, 0, bits, s);
-        TRY(c->cub_tmp.ensure(tb));
-        tb = c->cub_tmp.cap;
-        CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tb, pk, c->sortkey2.p, c->ids.p, c->inv.p, (int)lnv, 0, bits, s));
-        tb = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tb, c->deg_new.p, c->rowptr2.p, (int)lnv + 1, s);
-        TRY(c->cub_tmp.ensure(tb));
-        tb = c->cub_tmp.cap;
-        CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, c->deg_new.p, c->rowptr2.p, (int)lnv + 1, s));
-        k_permute_adj<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->perm.p, c->inv.p, src_rowptr, src_tails, src_weights,
-                                                               c->rowptr2.p, c->tails2.p, c->unit ? nullptr : c->weights2.p,
-                                                               (int)c->roff[c->rank], &d_sc->unordered);
-        c->tm.kernel_launches += 3;
-        src_rowptr = c->rowptr2.p;
-        src_tails = c->tails2.p;
-        src_weights = c->unit ? nullptr : c->weights2.p;
-        c->reordered = true;
-      }
-      CK(cudaEventRecord(r1, s));
-    }
-    // peers asked for my vertices by ORIGINAL id: the send list holds their current (internal) local index
-    if (c->relabel && c->nsend) {
-      k_apply_inv<<<grid_for(c->nsend, 256, nsm), 256, 0, s>>>(c->send_lid.p, (int)c->nsend, c->inv.p);
-      c->tm.kernel_launches++;
-    }
+  c->lay = LayoutReport();
+  c->lay.tails = g.tails;
+  int want = !ev && c->opt_reorder == 1 ? 1 : 0;
+  if (!ev && c->opt_reorder == 2 && lnv >= 65536) {
+    // auto: renumber when the given numbering has no locality (mean |tail - v| above lnv/64 on a vertex sample)
+    k_span_sample<<<grid_for(lnv / 64 + 1, 256, nsm), 256, 0, s>>>((int)lnv, g.rowptr, g.tails, 64, &d_sc->span_sum, &d_sc->span_cnt);
+    c->tm.kernel_launches++;
+    unsigned long long sp2[2];
+    CK(cudaMemcpyAsync(sp2, &d_sc->span_sum, sizeof sp2, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (sp2[1] > 0 && (double)sp2[0] / (double)sp2[1] > (double)lnv / 64.0) want = 1;
+    c->lay.span[0] = (long long)sp2[0]; c->lay.span[1] = (long long)sp2[1];
   }
+  // region ids have kBfsRegionBits bits: past 2^22 - 1 regions they would spill into the level field (and region
+  // 2^22 - 1 at level 1023 would read as kBfsUnreached), so very large shards get proportionally larger regions
+  const int stride = (int)std::max<long long>(c->opt_region, (lnv + kBfsMaxRegions - 1) / kBfsMaxRegions);
+  c->lay.want = want;
+  c->lay.stride = stride;
+  int any = want;
+  if (c->nranks > 1) {
+    long long hv = want;
+    TRY(coll_allreduce_i64(c, &hv, 1, true));
+    any = hv != 0;
+  }
+  c->relabel = any;                         // labels are needed everywhere as soon as one rank renumbers
+  if (any && lnv > 0) {
+    cudaEvent_t r0 = get_event(c, 2), r1 = get_event(c, 3);
+    CK(cudaEventRecord(r0, s));
+    TRY(c->perm.ensure(lnv)); TRY(c->inv.ensure(lnv)); TRY(c->lab.ensure(lnv)); TRY(c->ids.ensure(lnv));
+    TRY(c->bfs_key.ensure(lnv)); TRY(c->sortkey.ensure(lnv)); TRY(c->sortkey2.ensure(std::max(lnv, 4 * ((lnv + 31) / 32))));
+    TRY(c->deg_new.ensure(lnv + 1)); TRY(c->rowptr2.ensure(lnv + 1 + 40)); TRY(c->tails2.ensure(lne + 4));
+    if (!c->unit) TRY(c->weights2.ensure(lne + 4));
+    const int max_levels = 1023;
+    if (want) {
+      TRY(c->bfs_level_count.ensure(max_levels));
+      int occ = 0;
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_msbfs, 256, 0));
+      if (occ < 1) return fail("k_msbfs cannot be made resident");
+      int ilnv = (int)lnv, st = stride, ml = max_levels;
+      const uint32_t *rp = g.rowptr; const int32_t *tl = g.tails; uint32_t *key = c->bfs_key.p;
+      // the BFS queue and its level bitmaps (4 bits per vertex) live in ids and sortkey2, which k_bfs_sortkeys and the
+      // sort only write after the BFS
+      int32_t *q = c->ids.p; unsigned int *lc = c->bfs_level_count.p; uint32_t *lm = c->sortkey2.p;
+      void *args[] = {&ilnv, &rp, &tl, &key, &st, &ml, &q, &lc, &lm};
+      CK(cudaLaunchCooperativeKernel((void *)k_msbfs, dim3(occ * nsm), dim3(256), args, 0, s));
+      // sort by (region, level): only the bits that can be set take part (one radix pass less than a 32-bit sort)
+      const long long nregions = (lnv + stride - 1) / stride;
+      c->lay.nregions = nregions;
+      int sort_bits = (int)kBfsLevelBits;
+      while ((1LL << (sort_bits - (int)kBfsLevelBits)) <= nregions && sort_bits < 32) sort_bits++;
+      const unsigned int unreached_key = sort_bits >= 32 ? 0xFFFFFFFFu : ((1u << sort_bits) - 1u);
+      k_bfs_sortkeys<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->bfs_key.p, c->sortkey.p, c->ids.p, unreached_key);
+      TRY(cub_run(c, [&](void *t, size_t &tb) {
+        return cub::DeviceRadixSort::SortPairs(t, tb, c->sortkey.p, c->sortkey2.p, c->ids.p, c->perm.p, (int)lnv, 0, sort_bits, s); }));
+      c->tm.kernel_launches += 3;
+    } else {
+      // another rank renumbers, this one keeps its order: identity permutation, labels still required
+      k_bfs_sortkeys<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->bfs_key.p, c->sortkey.p, c->perm.p, 0xFFFFFFFFu);
+      c->tm.kernel_launches++;
+    }
+    k_perm_inverse<<<grid_for(lnv + 1, 256, nsm), 256, 0, s>>>((int)lnv, c->perm.p, c->base, want ? nullptr : c->inv.p, c->lab.p, g.rowptr, c->deg_new.p);
+    c->tm.kernel_launches++;
+    if (want) {
+      // inv[old] = new as a second radix sort (keys perm, values the ids 0..lnv-1 still in c->ids): lnv random 4-byte
+      // stores inv[perm[i]] = i cost more than twice as much as the sort's bucketed scatters (DESIGN.md §3.3)
+      int bits = 1;
+      while ((1LL << bits) < lnv && bits < 31) bits++;
+      const uint32_t *pk = reinterpret_cast<const uint32_t *>(c->perm.p);
+      TRY(cub_run(c, [&](void *t, size_t &tb) {
+        return cub::DeviceRadixSort::SortPairs(t, tb, pk, c->sortkey2.p, c->ids.p, c->inv.p, (int)lnv, 0, bits, s); }));
+      TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, c->deg_new.p, c->rowptr2.p, (int)lnv + 1, s); }));
+      k_permute_adj<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->perm.p, c->inv.p, g.rowptr, g.tails, g.weights,
+                                                             c->rowptr2.p, c->tails2.p, c->unit ? nullptr : c->weights2.p,
+                                                             (int)c->roff[c->rank], &d_sc->unordered);
+      c->tm.kernel_launches += 3;
+      g.rowptr = c->rowptr2.p;
+      g.tails = c->tails2.p;
+      g.weights = c->unit ? nullptr : c->weights2.p;
+      c->reordered = true;
+    }
+    CK(cudaEventRecord(r1, s));
+  }
+  // peers asked for my vertices by ORIGINAL id: the send list holds their current (internal) local index
+  if (c->relabel && c->nsend) {
+    k_apply_inv<<<grid_for(c->nsend, 256, nsm), 256, 0, s>>>(c->send_lid.p, (int)c->nsend, c->inv.p);
+    c->tm.kernel_launches++;
+  }
+  return 0;
+}
 
-  c->a_rowptr = src_rowptr; c->a_tails = src_tails; c->a_weights = src_weights;
-
-  // state arrays
+// state arrays and the singleton start (k_vertex_init) over the compact CSR in c->a_*
+int init_state(mvgpu_ctx *c, const EvalSetup *ev, long long nremote) {
+  cudaStream_t s = c->stream; const int nsm = c->num_sms; Scalars *d_sc = dev_scalars(c);
+  const long long lnv = c->lnv;
   // sized for the bound the collective "does an exported array have to grow?" test can evaluate before the ghosts are
   // known (lnv + #non-owned edge tails >= lnv + nghost), so that a repeated run never looks like a growing one
   const long long nslots = lnv + c->nghost;
@@ -836,7 +875,6 @@ int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
     TRY(c->q_internal.ensure(lnv)); TRY(c->q_rank.ensure(lnv + 1));
     CK(cudaMemsetAsync(c->q_internal.p, 0, sizeof(double) * lnv, s));
   }
-
   if (c->unit)
     k_vertex_init<true><<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->base, c->a_rowptr, c->a_tails, nullptr, c->comm_a.p,
                                                               c->cdeg.p, c->csize.p, c->upd.p, nullptr, nullptr, nullptr, nullptr,
@@ -850,60 +888,94 @@ int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
   // ghosts start in their own (internal) singleton community, which only the owner knows after renumbering:
   // fetch it with the same all-to-all-v the iterations use (a warm run fills comm_a in warm_init instead)
   if (c->nranks > 1 && !c->warm_run) TRY(exchange_ghosts(c, c->comm_a.p));
+  return 0;
+}
 
-  // high-degree vertices
-  // largest degree the tile kernels take: one staging buffer (minus the 16-byte alignment slack of the bulk copies)
+// high-degree vertices, launched here and listed by heavy_finish after the 1/(2m) read-back.  heavy_deg: the largest
+// degree the tile kernels take, one staging buffer (minus the 16-byte alignment slack of the bulk copies)
+int heavy_launch(mvgpu_ctx *c, long long &heavy_deg) {
   const long long tile_cap = c->opt_scan_variant >= 4 ? (c->unit ? PwCap<true>::value : PwCap<false>::value) - 4 : kECap;
-  const long long heavy_deg = (c->opt_force_heavy_deg > 0) ? std::min<long long>(c->opt_force_heavy_deg, tile_cap) : tile_cap;
+  heavy_deg = (c->opt_force_heavy_deg > 0) ? std::min<long long>(c->opt_force_heavy_deg, tile_cap) : tile_cap;
   c->nheavy = 0;
   if (c->maxdeg > heavy_deg) {
-    TRY(c->heavy_list.ensure(lnv));
-    k_collect_heavy<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->a_rowptr, (unsigned int)heavy_deg, c->heavy_list.p, &d_sc->heavy_count);
+    TRY(c->heavy_list.ensure(c->lnv));
+    k_collect_heavy<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>((int)c->lnv, c->a_rowptr, (unsigned int)heavy_deg, c->heavy_list.p,
+                                                                              &dev_scalars(c)->heavy_count);
     c->tm.kernel_launches++;
   }
+  return 0;
+}
 
-  // 1/(2m): MPI_Allreduce of the local degree sums (dspl.hpp:109-130)
+// 1/(2m): MPI_Allreduce of the local degree sums (dspl.hpp:109-130), read back with the flags of k_vertex_init into h
+int total_weight(mvgpu_ctx *c, Scalars &h) {
+  cudaStream_t s = c->stream; Scalars *d_sc = dev_scalars(c);
   if (c->nranks > 1 && !c->hc.is_open()) NK(g_nccl.AllReduce(&d_sc->total_weight, &d_sc->total_weight, 1, ncclDouble, ncclSum, c->comm, s));
   CK(cudaMemcpyAsync(&h, d_sc, sizeof h, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (c->nranks > 1 && c->hc.is_open()) c->hc.allreduce(&h.total_weight, 1, [](double a, double b) { return a + b; });
   c->constant = 1.0 / h.total_weight;
   if (c->f32) c->constant = (double)(float)(1.0 / (double)(float)h.total_weight);   // dspl.hpp:129 with GraphWeight = float
-  const int has_self = h.has_self ? 1 : 0;
-  c->simple_sorted = c->unit && !h.unordered && !has_self;
-  c->lay_unordered = h.unordered ? 1 : 0;
-  c->lay_has_self = has_self;
-  if (c->maxdeg > heavy_deg) {
-    c->nheavy = h.heavy_count;
-    std::vector<int32_t> hl(c->nheavy);
-    CK(cudaMemcpy(hl.data(), c->heavy_list.p, sizeof(int32_t) * c->nheavy, cudaMemcpyDeviceToHost));
-    std::sort(hl.begin(), hl.end());
-    CK(cudaMemcpy(c->heavy_list.p, hl.data(), sizeof(int32_t) * c->nheavy, cudaMemcpyHostToDevice));
-    std::vector<unsigned long long> off(c->nheavy + 1, 0);
-    for (long long i = 0; i < c->nheavy; i++) {
-      uint32_t r2[2];
-      CK(cudaMemcpy(r2, c->a_rowptr + hl[i], sizeof r2, cudaMemcpyDeviceToHost));
-      unsigned long long T = 64;
-      while (T < 2ULL * (r2[1] - r2[0])) T <<= 1;
-      off[i + 1] = off[i] + T;
-    }
-    TRY(c->heavy_off.ensure(c->nheavy + 1));
-    CK(cudaMemcpy(c->heavy_off.p, off.data(), sizeof(unsigned long long) * (c->nheavy + 1), cudaMemcpyHostToDevice));
-    TRY(c->hkeys.ensure(off[c->nheavy]));
-    if (c->unit) TRY(c->hvals_i.ensure(off[c->nheavy])); else TRY(c->hvals_d.ensure(off[c->nheavy]));
-  }
-  if (c->nranks > 1) {
-    TRY(c->p2p.ensure(1));
-    if (!c->p2p_zeroed) { CK(cudaMemsetAsync(c->p2p.p, 0, sizeof(P2PState), s)); CK(cudaStreamSynchronize(s)); c->p2p_zeroed = true; }
-  }
-  TRY(setup_peers(c, c->unit ? 1 : 0));
-  if (c->warm_run) TRY(warm_init(c, ev ? ev->X : c->init_comm.p));
-  c->tm.unit_weight = c->unit ? 1 : 0;
-  c->scan_has_self = has_self;
-  c->scan_heavy_deg = (int)heavy_deg;
+  c->lay.has_self = h.has_self ? 1 : 0;
+  c->lay.unordered = h.unordered ? 1 : 0;
+  c->simple_sorted = c->unit && !h.unordered && !h.has_self;
   return 0;
 }
 
+// high-degree vertices, second half: the sorted list and each one's hash-table offset
+int heavy_finish(mvgpu_ctx *c, long long heavy_deg, unsigned int heavy_count) {
+  if (c->maxdeg <= heavy_deg) return 0;
+  c->nheavy = heavy_count;
+  std::vector<int32_t> hl(c->nheavy);
+  CK(cudaMemcpy(hl.data(), c->heavy_list.p, sizeof(int32_t) * c->nheavy, cudaMemcpyDeviceToHost));
+  std::sort(hl.begin(), hl.end());
+  CK(cudaMemcpy(c->heavy_list.p, hl.data(), sizeof(int32_t) * c->nheavy, cudaMemcpyHostToDevice));
+  std::vector<unsigned long long> off(c->nheavy + 1, 0);
+  for (long long i = 0; i < c->nheavy; i++) {
+    uint32_t r2[2];
+    CK(cudaMemcpy(r2, c->a_rowptr + hl[i], sizeof r2, cudaMemcpyDeviceToHost));
+    unsigned long long T = 64;
+    while (T < 2ULL * (r2[1] - r2[0])) T <<= 1;
+    off[i + 1] = off[i] + T;
+  }
+  TRY(c->heavy_off.ensure(c->nheavy + 1));
+  CK(cudaMemcpy(c->heavy_off.p, off.data(), sizeof(unsigned long long) * (c->nheavy + 1), cudaMemcpyHostToDevice));
+  TRY(c->hkeys.ensure(off[c->nheavy]));
+  if (c->unit) TRY(c->hvals_i.ensure(off[c->nheavy])); else TRY(c->hvals_d.ensure(off[c->nheavy]));
+  return 0;
+}
+
+// ev != nullptr: setup for an evaluation -- warm init from ev->X, no locality renumbering, evaluation arrays allocated
+int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
+  TRY(c->scratch.ensure(sizeof(Scalars)));
+  CK(cudaMemsetAsync(c->scratch.p, 0, sizeof(Scalars), c->stream));
+  c->warm_run = ev ? true : c->have_init;
+  Scalars h;                                  // the device scalars after the input pass, then after the 1/(2m) read-back
+  int unit = 0;
+  std::string err;
+  TRY(input_pass(c, ev, h, unit, err));
+  const long long nremote = (long long)h.st.nremote;
+  TRY(setup_agree(c, ev, nremote, unit, err));
+  Csr g;
+  TRY(compact_edges(c, nremote, g));
+  TRY(discover_ghosts(c, nremote));
+  TRY(renumber(c, ev, g));
+  c->a_rowptr = g.rowptr; c->a_tails = g.tails; c->a_weights = g.weights;
+  TRY(init_state(c, ev, nremote));
+  long long heavy_deg = 0;
+  TRY(heavy_launch(c, heavy_deg));
+  TRY(total_weight(c, h));
+  TRY(heavy_finish(c, heavy_deg, h.heavy_count));
+  if (c->nranks > 1) {
+    TRY(c->p2p.ensure(1));
+    if (!c->p2p_zeroed) { CK(cudaMemsetAsync(c->p2p.p, 0, sizeof(P2PState), c->stream)); CK(cudaStreamSynchronize(c->stream)); c->p2p_zeroed = true; }
+  }
+  TRY(setup_peers(c));
+  if (c->warm_run) TRY(warm_init(c, ev ? ev->X : c->init_comm.p));
+  c->tm.unit_weight = c->unit ? 1 : 0;
+  c->scan_has_self = c->lay.has_self;
+  c->scan_heavy_deg = (int)heavy_deg;
+  return 0;
+}
 
 // ---- ghost exchange: targetComm of the vertices peers ghost -> ghost tail of their community array.
 // The reference's gather + Isend/Irecv/Waitall (dspl.hpp:559-646) as one grouped NCCL all-to-all-v with
@@ -926,6 +998,53 @@ int check_ready(mvgpu_ctx *c) {
   return 0;
 }
 
+// ---- the cross-rank sum of an Acc record (dspl.hpp:441): e and a2 in rank order, plus the trace counters.
+// acc_sum_enqueue puts it on the stream, into the pinned mailbox; acc_sum_read reads it after the caller's synchronise.
+struct HostMail { Acc acc; double red2[2]; unsigned long long tr2[2]; unsigned int p2p_error; };
+struct AccSum { double e, a2; unsigned long long moved, hash; };
+
+int acc_sum_enqueue(mvgpu_ctx *c, Acc *acc, bool trace) {
+  cudaStream_t s = c->stream; Scalars *d_sc = dev_scalars(c);
+  HostMail *mail = reinterpret_cast<HostMail *>(c->h_pin);
+  if (c->nranks == 1) CK(cudaMemcpyAsync(&mail->acc, acc, sizeof(Acc), cudaMemcpyDeviceToHost, s));
+  else if (c->opt_comm_mode == 1) {
+    k_p2p_allreduce<<<1, 32, 0, s>>>(c->pp, ++c->p2p_epoch, acc, c->unit ? 1 : 0, d_sc->red2, d_sc->tr2);
+    c->tm.kernel_launches++;
+    CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2 + sizeof mail->tr2, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&mail->p2p_error, &c->p2p.p->error, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+  } else {
+    k_acc_to_double<<<1, 32, 0, s>>>(acc, c->unit ? 1 : 0, d_sc->red2);
+    c->tm.kernel_launches++;
+    NK(g_nccl.AllReduce(d_sc->red2, d_sc->red2, 2, ncclDouble, ncclSum, c->comm, s));
+    CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2, cudaMemcpyDeviceToHost, s));
+    if (trace) {
+      k_trace_to_u64<<<1, 32, 0, s>>>(acc, d_sc->tr2);
+      c->tm.kernel_launches++;
+      NK(g_nccl.AllReduce(d_sc->tr2, d_sc->tr2, 2, ncclUint64, ncclSum, c->comm, s));
+      CK(cudaMemcpyAsync(mail->tr2, d_sc->tr2, sizeof mail->tr2, cudaMemcpyDeviceToHost, s));
+    }
+  }
+  return 0;
+}
+
+// moved / hash are only summed over several NCCL ranks when acc_sum_enqueue was asked for the trace
+int acc_sum_read(mvgpu_ctx *c, AccSum &r) {
+  const HostMail *mail = reinterpret_cast<const HostMail *>(c->h_pin);
+  const Acc &a = mail->acc;
+  if (c->nranks == 1) r = {c->unit ? (double)a.le_u : a.le_d, c->unit ? (double)a.la2_u : a.la2_d, a.moved, a.hash};
+  else if (c->opt_comm_mode == 1 && mail->p2p_error) return fail("peer-memory collective timed out (a peer rank is gone)");
+  else r = {mail->red2[0], mail->red2[1], mail->tr2[0], mail->tr2[1]};
+  return 0;
+}
+
+// Q = e * constant - a2 * constant * constant with every product rounded on its own (dspl.hpp:447-448)
+double modularity(double e, double a2, double cst) {
+  volatile double term1 = e * cst;
+  volatile double term2a = a2 * cst;
+  volatile double term2 = term2a * cst;
+  return term1 - term2;
+}
+
 int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, double *mod_out) {
   TRY(check_ready(c));
   CK(cudaSetDevice(c->device));
@@ -940,7 +1059,6 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   TRY(setup_run(c));
   CK(cudaEventRecord(e_setup, s));
 
-  Scalars *d_sc = reinterpret_cast<Scalars *>(c->scratch.p);
   int32_t *cur = c->comm_a.p, *tgt = c->comm_b.p;
   ScanParams sp;
   memset(&sp, 0, sizeof sp);
@@ -955,8 +1073,6 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   sp.loc_usize = c->usize.p; sp.loc_udeg = c->udeg.p; sp.loc_lab = c->relabel ? c->lab.p : nullptr;
   c->last_sp = sp;
 
-  struct HostMail { Acc acc; double red2[2]; unsigned long long tr2[2]; unsigned int p2p_error; };
-  HostMail *mail = reinterpret_cast<HostMail *>(c->h_pin);
   const size_t ev_iter0 = ev;
   double prevMod = lower, currMod = -1.0;
   int numIters = 0, auto_choice = 4;
@@ -997,7 +1113,7 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
         c->tm.kernel_launches++;
       } else {
         TRY(exchange_ghosts(c, tgt));
-        NK(g_nccl.AllReduce(d_sc->counts, d_sc->counts, 1, ncclInt64, ncclSum, c->comm, s));
+        NK(g_nccl.AllReduce(dev_scalars(c)->counts, dev_scalars(c)->counts, 1, ncclInt64, ncclSum, c->comm, s));
       }
     }
     CK(cudaEventRecord(e2, s));
@@ -1005,38 +1121,10 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
     else k_fold_w<<<fold_grid, 256, 0, s>>>((int)c->lnv, c->cinfo_w.p, c->usize.p, c->udeg.p, acc);
     c->tm.kernel_launches++;
     CK(cudaEventRecord(e3, s));
-    double e_xx, a2_x;
-    unsigned long long moved = 0, hash = 0;
-    if (p2p) {
-      k_p2p_allreduce<<<1, 32, 0, s>>>(c->pp, ++c->p2p_epoch, acc, c->unit ? 1 : 0, d_sc->red2, d_sc->tr2);   // dspl.hpp:441
-      c->tm.kernel_launches++;
-      CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2 + sizeof mail->tr2, cudaMemcpyDeviceToHost, s));
-      CK(cudaMemcpyAsync(&mail->p2p_error, &c->p2p.p->error, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      if (mail->p2p_error) return fail("peer-memory collective timed out (a peer rank is gone)");
-      e_xx = mail->red2[0]; a2_x = mail->red2[1];
-      moved = mail->tr2[0]; hash = mail->tr2[1];
-    } else if (c->nranks > 1) {
-      k_acc_to_double<<<1, 32, 0, s>>>(acc, c->unit ? 1 : 0, d_sc->red2);
-      c->tm.kernel_launches++;
-      NK(g_nccl.AllReduce(d_sc->red2, d_sc->red2, 2, ncclDouble, ncclSum, c->comm, s));   // dspl.hpp:441
-      CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2, cudaMemcpyDeviceToHost, s));
-      if (c->opt_trace) {
-        k_trace_to_u64<<<1, 32, 0, s>>>(acc, d_sc->tr2);
-        c->tm.kernel_launches++;
-        NK(g_nccl.AllReduce(d_sc->tr2, d_sc->tr2, 2, ncclUint64, ncclSum, c->comm, s));
-        CK(cudaMemcpyAsync(mail->tr2, d_sc->tr2, sizeof mail->tr2, cudaMemcpyDeviceToHost, s));
-      }
-      CK(cudaStreamSynchronize(s));
-      e_xx = mail->red2[0]; a2_x = mail->red2[1];
-      moved = mail->tr2[0]; hash = mail->tr2[1];
-    } else {
-      CK(cudaMemcpyAsync(&mail->acc, acc, sizeof(Acc), cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      e_xx = c->unit ? (double)mail->acc.le_u : mail->acc.le_d;
-      a2_x = c->unit ? (double)mail->acc.la2_u : mail->acc.la2_d;
-      moved = mail->acc.moved; hash = mail->acc.hash;
-    }
+    TRY(acc_sum_enqueue(c, acc, c->opt_trace != 0));
+    CK(cudaStreamSynchronize(s));
+    AccSum sum;
+    TRY(acc_sum_read(c, sum));
     if (c->opt_scan_variant == 6 && numIters == 4) {           // iterations 2..4 have completed (the stream was just synchronised)
       float t2 = 0, t3 = 0, t4 = 0;
       CK(cudaEventElapsedTime(&t2, c->events[ev_iter0 + 4 * 1], c->events[ev_iter0 + 4 * 1 + 1]));
@@ -1045,24 +1133,19 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
       auto_choice = ((double)t3 * t3 < (double)t2 * t4) ? 5 : 4;
       c->tm.scan_kernel_chosen = auto_choice;
     }
-    // dspl.hpp:447-448
-    const double cst = c->constant;
     if (c->f32) {                      // GraphWeight = float: every product and the difference round to float
-      const float cf = (float)cst;
-      volatile float t1f = (float)e_xx * cf;
-      volatile float t2af = (float)a2_x * cf;
+      const float cf = (float)c->constant;
+      volatile float t1f = (float)sum.e * cf;
+      volatile float t2af = (float)sum.a2 * cf;
       volatile float t2f = t2af * cf;
       volatile float df = t1f - t2f;
       currMod = (double)std::fabs(df);
     } else {
-    volatile double term1 = e_xx * cst;
-    volatile double term2a = a2_x * cst;
-    volatile double term2 = term2a * cst;
-    currMod = std::fabs(term1 - term2);
+      currMod = std::fabs(modularity(sum.e, sum.a2, c->constant));
     }
     if (c->opt_trace) {
       mvgpu_iter_trace t;
-      t.modularity = currMod; t.moved = (int64_t)moved; t.chash = hash;
+      t.modularity = currMod; t.moved = (int64_t)sum.moved; t.chash = sum.hash;
       c->trace.push_back(t);
     }
     if (c->f32 ? ((float)currMod - (float)prevMod < (float)thresh) : (currMod - prevMod < thresh)) break;   // dspl.hpp:1401-1402
@@ -1082,8 +1165,7 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
     // free its arrays (mvgpu_destroy) without a peer still reading them.  Outside the timed region, like the
     // reference's output code is outside its timer.
     TRY(final_in_caller_order(c));
-    if (c->opt_comm_mode == 1) { k_p2p_barrier<<<1, 32, 0, s>>>(c->pp, ++c->p2p_epoch); c->tm.kernel_launches++; }
-    else TRY(coll_barrier(c));
+    TRY(run_barrier(c));
     CK(cudaStreamSynchronize(s));
   }
   CK(cudaEventSynchronize(e_end));
@@ -1129,28 +1211,24 @@ __global__ void k_widen(const int32_t *in, long long n, long long *out) {
 // keeps a copy and puts it back.
 struct RunReport {
   mvgpu_timings tm;
+  LayoutReport lay;
   double constant;
-  bool reordered, simple_sorted, unit, warm_run, lay_first_ran;
-  int relabel, lay_want, lay_stride, lay_unordered, lay_has_self;
-  long long lay_nregions, lay_span[2];
-  const int32_t *lay_tails;
+  bool reordered, simple_sorted, unit, warm_run;
+  int relabel;
 };
 RunReport save_report(const mvgpu_ctx *c) {
-  return {c->tm, c->constant, c->reordered, c->simple_sorted, c->unit, c->warm_run, c->lay_first_ran, c->relabel, c->lay_want,
-          c->lay_stride, c->lay_unordered, c->lay_has_self, c->lay_nregions, {c->lay_span[0], c->lay_span[1]}, c->lay_tails};
+  return {c->tm, c->lay, c->constant, c->reordered, c->simple_sorted, c->unit, c->warm_run, c->relabel};
 }
 void restore_report(mvgpu_ctx *c, const RunReport &r) {
-  c->tm = r.tm; c->constant = r.constant; c->reordered = r.reordered; c->simple_sorted = r.simple_sorted; c->unit = r.unit;
-  c->warm_run = r.warm_run; c->lay_first_ran = r.lay_first_ran; c->relabel = r.relabel; c->lay_want = r.lay_want;
-  c->lay_stride = r.lay_stride; c->lay_unordered = r.lay_unordered; c->lay_has_self = r.lay_has_self;
-  c->lay_nregions = r.lay_nregions; c->lay_span[0] = r.lay_span[0]; c->lay_span[1] = r.lay_span[1]; c->lay_tails = r.lay_tails;
+  c->tm = r.tm; c->lay = r.lay; c->constant = r.constant; c->reordered = r.reordered; c->simple_sorted = r.simple_sorted;
+  c->unit = r.unit; c->warm_run = r.warm_run; c->relabel = r.relabel;
 }
 
 // ---- evaluation (DESIGN.md §3.10): after setup_run(ev), comm_a = X on every slot and the Comm records are X's -------
 int evaluate_pass(mvgpu_ctx *c, const int32_t *X, mvgpu_quality *out) {
   cudaStream_t s = c->stream;
   const int lnv = (int)c->lnv, nsm = c->num_sms;
-  Scalars *d_sc = reinterpret_cast<Scalars *>(c->scratch.p);
+  Scalars *d_sc = dev_scalars(c);
   Acc *acc0 = c->acc.p;                        // warm_init left a2 (unit path) in record 0; e_in joins it there
   if (!c->unit) {                              // the update arrays are zero after the warm fold: this only sums a_c^2
     k_fold_w<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->cinfo_w.p, c->usize.p, c->udeg.p, acc0);
@@ -1162,21 +1240,8 @@ int evaluate_pass(mvgpu_ctx *c, const int32_t *X, mvgpu_quality *out) {
     k_q_internal<false><<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->a_rowptr, c->a_tails, c->a_weights, c->comm_a.p, c->pt, c->qp, acc0);
   c->tm.kernel_launches++;
   TRY(run_barrier(c));                         // every rank's internal-weight adds have landed in the owners' records
-  // e_in and a2, summed over the ranks in rank order like the run's modularity partials (dspl.hpp:441)
-  struct HostMail { Acc acc; double red2[2]; unsigned long long tr2[2]; unsigned int p2p_error; };
-  HostMail *mail = reinterpret_cast<HostMail *>(c->h_pin);
-  if (c->nranks > 1 && c->opt_comm_mode == 1) {
-    k_p2p_allreduce<<<1, 32, 0, s>>>(c->pp, ++c->p2p_epoch, acc0, c->unit ? 1 : 0, d_sc->red2, d_sc->tr2);
-    c->tm.kernel_launches++;
-    CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2, cudaMemcpyDeviceToHost, s));
-  } else if (c->nranks > 1) {
-    k_acc_to_double<<<1, 32, 0, s>>>(acc0, c->unit ? 1 : 0, d_sc->red2);
-    c->tm.kernel_launches++;
-    NK(g_nccl.AllReduce(d_sc->red2, d_sc->red2, 2, ncclDouble, ncclSum, c->comm, s));
-    CK(cudaMemcpyAsync(mail->red2, d_sc->red2, sizeof mail->red2, cudaMemcpyDeviceToHost, s));
-  } else {
-    CK(cudaMemcpyAsync(&mail->acc, acc0, sizeof(Acc), cudaMemcpyDeviceToHost, s));
-  }
+  // e_in and a2, summed over the ranks in rank order like the run's modularity partials
+  TRY(acc_sum_enqueue(c, acc0, false));
   // per-community arrays, non-empty flags in owned slot order (= caller id order: no renumbering), their exclusive sum
   TRY(c->q_flag.ensure(lnv + 1)); TRY(c->q_size.ensure(lnv)); TRY(c->q_vol.ensure(lnv)); TRY(c->q_lab.ensure(lnv));
   CK(cudaMemsetAsync(d_sc->q_agg, 0, sizeof d_sc->q_agg, s));
@@ -1186,22 +1251,15 @@ int evaluate_pass(mvgpu_ctx *c, const int32_t *X, mvgpu_quality *out) {
   else
     k_q_stats<false><<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, nullptr, nullptr, c->cinfo_w.p, c->q_internal.p, c->q_size.p, c->q_vol.p,
                                                              c->q_flag.p, d_sc->q_agg);
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, c->q_flag.p, c->q_rank.p, lnv + 1, s);
-  TRY(c->cub_tmp.ensure(tb));
-  tb = c->cub_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, c->q_flag.p, c->q_rank.p, lnv + 1, s));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, c->q_flag.p, c->q_rank.p, lnv + 1, s); }));
   c->tm.kernel_launches += 2;
   int32_t nonempty = 0;
   unsigned long long agg[2];
   CK(cudaMemcpyAsync(&nonempty, c->q_rank.p + lnv, sizeof nonempty, cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(agg, d_sc->q_agg, sizeof agg, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (c->nranks > 1 && c->opt_comm_mode == 1) {
-    unsigned int err = 0;
-    CK(cudaMemcpy(&err, &c->p2p.p->error, sizeof err, cudaMemcpyDeviceToHost));
-    if (err) return fail("peer-memory collective timed out (a peer rank is gone)");
-  }
+  AccSum sum;
+  TRY(acc_sum_read(c, sum));
   // rank offsets of the compact labels: every rank's {non-empty, singletons, largest}; each rank's prefix sum is
   // complete before it contributes, so the owners' arrays are final when the gather below reads them
   std::vector<long long> all(3 * (size_t)c->nranks);
@@ -1222,17 +1280,23 @@ int evaluate_pass(mvgpu_ctx *c, const int32_t *X, mvgpu_quality *out) {
     CK(cudaStreamSynchronize(s));
   }
   CK(cudaGetLastError());
-  const double e = c->nranks > 1 ? mail->red2[0] : (c->unit ? (double)mail->acc.le_u : mail->acc.le_d);
-  const double a2 = c->nranks > 1 ? mail->red2[1] : (c->unit ? (double)mail->acc.la2_u : mail->acc.la2_d);
-  const double cst = c->constant;              // run_louvain's rounding (dspl.hpp:447-448), without the fabs
-  volatile double term1 = e * cst;
-  volatile double term2a = a2 * cst;
-  volatile double term2 = term2a * cst;
-  out->modularity = term1 - term2;
-  out->e_in = e; out->a2 = a2; out->constant = cst;
+  out->modularity = modularity(sum.e, sum.a2, c->constant);   // run_louvain's rounding, without the fabs
+  out->e_in = sum.e; out->a2 = sum.a2; out->constant = c->constant;
   out->communities = communities; out->singletons = singletons; out->max_size = max_size;
   c->eval_on_shard = true;
   return 0;
+}
+
+// the caller's community ids (lnv of them) as int32 in h; what is wrong with them ("" if nothing), prefixed by `who`
+std::string narrow_ids(const mvgpu_ctx *c, const int64_t *comm, const char *who, std::vector<int32_t> &h) {
+  h.resize((size_t)c->lnv);
+  for (long long i = 0; i < c->lnv; i++) {
+    if (comm[i] < 0 || comm[i] >= c->nv_global)
+      return std::string(who) + ": community id " + std::to_string((long long)comm[i]) + " of local vertex " + std::to_string(i) +
+             " outside [0, nv)";
+    h[i] = (int32_t)comm[i];
+  }
+  return "";
 }
 
 // collective: every rank calls it with an array or every rank with NULL.  caller_err: a finding of the caller's own
@@ -1253,13 +1317,8 @@ int evaluate(mvgpu_ctx *c, const int64_t *comm, mvgpu_quality *out, const char *
   else if (c->f32) ev.err = "mvgpu_evaluate_communities: not for a shard uploaded with mvgpu_upload_shard32";
   else if (!comm && !c->run_on_shard) ev.err = "mvgpu_evaluate_communities: NULL evaluates the last mvgpu_louvain result, and there is none on this shard";
   else if (comm) {
-    std::vector<int32_t> h((size_t)c->lnv);
-    for (long long i = 0; i < c->lnv && ev.err.empty(); i++) {
-      if (comm[i] < 0 || comm[i] >= c->nv_global)
-        ev.err = "mvgpu_evaluate_communities: community id " + std::to_string((long long)comm[i]) + " of local vertex " +
-                 std::to_string(i) + " outside [0, nv)";
-      h[i] = (int32_t)comm[i];
-    }
+    std::vector<int32_t> h;
+    ev.err = narrow_ids(c, comm, "mvgpu_evaluate_communities", h);
     if (ev.err.empty()) {
       TRY(c->eval_comm.ensure(c->lnv));
       if (c->lnv) CK(cudaMemcpyAsync(c->eval_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice, s));
@@ -1324,18 +1383,10 @@ static int add_random_edges(mvgpu_ctx *c, const RggParams &P, int64_t nv, int un
   CK(cudaMemcpyAsync(dsoff.p, soff.data(), sizeof(long long) * (p + 1), cudaMemcpyHostToDevice, s));
   k_rande_draws<<<p, 32, 0, s>>>(R, dsoff.p, di.p, dgj.p);
   k_rande_keys<<<grid_for(nrande, 256, nsm), 256, 0, s>>>(R, dsoff.p, di.p, dgj.p, nrande, c->gen_rowptr.p, c->gen_edges.p, key.p, qidx.p);
-  size_t tb = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tb, key.p, skey.p, qidx.p, sq.p, (int)nrande, 0, 64, s);
-  TRY(c->cub_tmp.ensure(tb));
-  tb = c->cub_tmp.cap;
-  CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tb, key.p, skey.p, qidx.p, sq.p, (int)nrande, 0, 64, s));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, key.p, skey.p, qidx.p, sq.p, (int)nrande, 0, 64, s); }));
   CK(cudaMemsetAsync(emit.p + nrande, 0, sizeof(unsigned int), s));
   k_rande_first<<<grid_for(nrande, 256, nsm), 256, 0, s>>>(skey.p, sq.p, nrande, R, dsoff.p, dgj.p, emit.p);
-  tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, emit.p, epos.p, (int)(nrande + 1), s);
-  TRY(c->cub_tmp.ensure(tb));
-  tb = c->cub_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, emit.p, epos.p, (int)(nrande + 1), s));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, emit.p, epos.p, (int)(nrande + 1), s); }));
   unsigned int nextra = 0;
   CK(cudaMemcpyAsync(&nextra, epos.p + nrande, sizeof nextra, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
@@ -1345,16 +1396,8 @@ static int add_random_edges(mvgpu_ctx *c, const RggParams &P, int64_t nv, int un
   CK(cudaMemsetAsync(add.p, 0, sizeof(unsigned int) * (P.n + 1), s));
   k_rande_emit<<<grid_for(nrande, 256, nsm), 256, 0, s>>>(R, P, dsoff.p, di.p, dgj.p, nrande, emit.p, epos.p, unit, X3, Y3, xkey.p, xw.p,
                                                         xidx.p, add.p);
-  tb = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tb, xkey.p, sxkey.p, xidx.p, sxidx.p, (int)nextra, 0, 62, s);
-  TRY(c->cub_tmp.ensure(tb));
-  tb = c->cub_tmp.cap;
-  CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tb, xkey.p, sxkey.p, xidx.p, sxidx.p, (int)nextra, 0, 62, s));
-  tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, add.p, xstart.p, (int)(P.n + 1), s);
-  TRY(c->cub_tmp.ensure(tb));
-  tb = c->cub_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, add.p, xstart.p, (int)(P.n + 1), s));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, xkey.p, sxkey.p, xidx.p, sxidx.p, (int)nextra, 0, 62, s); }));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, add.p, xstart.p, (int)(P.n + 1), s); }));
   k_rande_rowptr<<<grid_for(P.n + 1, 256, nsm), 256, 0, s>>>(c->gen_rowptr.p, xstart.p, P.n, nrow.p);
   const long long lne2 = *lne_io + (long long)nextra;
   DevBuf<Edge16> merged;
@@ -1426,29 +1469,15 @@ int mvgpu_destroy(mvgpu_ctx *c) {
   if (!c) return 0;
   cudaSetDevice(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
-  for (void *p : c->ipc_opened) cudaIpcCloseMemHandle(p);
+  close_ipc(c);
   if (c->comm) g_nccl.CommDestroy(c->comm);
   c->hc.close_comm();
   for (cudaEvent_t e : c->events) cudaEventDestroy(e);
   if (c->h_stage) cudaFreeHost(c->h_stage);
-  c->in_tails32.release(); c->wide.release(); c->raw_ring.release();
   for (int b = 0; b < 2; b++) if (c->h_bounce[b]) cudaFreeHost(c->h_bounce[b]);
-  c->gen_rowptr.release(); c->gen_edges.release();
-  c->in_rowptr.release(); c->in_edges.release(); c->rowptr.release(); c->tails.release(); c->weights.release();
-  c->self_i.release(); c->self_d.release(); c->vdeg.release(); c->comm_a.release(); c->comm_b.release();
-  c->cdeg.release(); c->csize.release(); c->upd.release(); c->cinfo_w.release(); c->usize.release(); c->udeg.release(); c->acc.release();
-  c->scratch.release(); c->cub_tmp.release(); c->coll_tmp.release(); c->sorted_tmp.release(); c->remote_list.release(); c->remote_pos.release(); c->ghost_gid.release(); c->send_gid.release();
-  c->bfs_key.release(); c->sortkey.release(); c->sortkey2.release(); c->deg_new.release(); c->rowptr2.release();
-  c->ids.release(); c->perm.release(); c->inv.release(); c->lab.release(); c->tails2.release(); c->final_orig.release();
-  c->weights2.release(); c->bfs_level_count.release();
-  c->p2p.release();
-  c->send_lid.release(); c->send_buf.release(); c->heavy_list.release(); c->hkeys.release(); c->hvals_i.release();
-  c->hvals_d.release(); c->heavy_off.release();
-  c->eval_comm.release(); c->q_internal.release(); c->q_vol.release(); c->q_rank.release(); c->q_flag.release();
-  c->q_lab.release(); c->q_size.release();
   if (c->h_pin) cudaFreeHost(c->h_pin);
   if (c->stream) cudaStreamDestroy(c->stream);
-  delete c;
+  delete c;                                    // the DevBufs free themselves
   return 0;
 }
 
@@ -1503,7 +1532,7 @@ static int upload_compact(mvgpu_ctx *c, int64_t nv_global, int64_t lne, const vo
   if (c->in_tails32.ensure(lne + 4)) return -1;
   if (c->raw_ring.ensure((size_t)2 * CH)) return -1;             // two raw chunks in flight on the device
   if (c->scratch.ensure(sizeof(Scalars))) return -1;
-  Scalars *d_sc = reinterpret_cast<Scalars *>(c->scratch.p);
+  Scalars *d_sc = dev_scalars(c);
   if (cudaMemsetAsync(&d_sc->st, 0, sizeof(EdgeStats), c->stream) != cudaSuccess) return -1;
   int32_t *stage = reinterpret_cast<int32_t *>(c->h_stage);
   const long long base = c->base, bound = c->bound;
@@ -1604,32 +1633,26 @@ int mvgpu_upload_shard(mvgpu_ctx *c, int64_t nv_global, const int64_t *parts, in
   if (!c || !parts || !edge_indices || (lne && !edge_list)) return fail("null argument");
   CK(cudaSetDevice(c->device));
   TRY(set_graph(c, nv_global, parts, lnv, lne));
-  c->f32 = false;
   TRY(c->in_rowptr.ensure(lnv + 1));
   cudaEvent_t a = get_event(c, 0), b = get_event(c, 1);
   CK(cudaEventRecord(a, c->stream));
   CK(cudaMemcpyAsync(c->in_rowptr.p, edge_indices, sizeof(long long) * (lnv + 1), cudaMemcpyHostToDevice, c->stream));
-  c->d_tails32 = nullptr;
-  c->d_edges = nullptr;
   int compact = 1;
   long long compact_bytes = 0;
   if (c->opt_compact_upload && !c->opt_force_weighted && lne > 0) {
     compact = upload_compact(c, nv_global, lne, edge_list, &compact_bytes);
     if (compact < 0) return fail(std::string("compact upload: ") + cudaGetErrorString(cudaGetLastError()));
   }
-  if (compact == 0) c->d_tails32 = c->in_tails32.p;
-  else {
+  if (compact != 0) {
     TRY(c->in_edges.ensure(lne));
     if (lne) CK(cudaMemcpyAsync(c->in_edges.p, edge_list, sizeof(Edge16) * lne, cudaMemcpyHostToDevice, c->stream));
-    c->d_edges = c->in_edges.p;
   }
   CK(cudaEventRecord(b, c->stream));
   CK(cudaEventSynchronize(b));
   float ms = 0;
   CK(cudaEventElapsedTime(&ms, a, b));
-  c->h2d_s = ms * 1e-3;
-  c->h2d_bytes = (long long)sizeof(long long) * (lnv + 1) + (compact == 0 ? compact_bytes : (long long)sizeof(Edge16) * lne);
-  c->d_rowptr64 = c->in_rowptr.p;
+  set_source(c, c->in_rowptr.p, compact == 0 ? nullptr : c->in_edges.p, compact == 0 ? c->in_tails32.p : nullptr, false, ms * 1e-3,
+             (long long)sizeof(long long) * (lnv + 1) + (compact == 0 ? compact_bytes : (long long)sizeof(Edge16) * lne));
   return 0;
 }
 
@@ -1639,12 +1662,7 @@ int mvgpu_attach_shard_device(mvgpu_ctx *c, int64_t nv_global, const int64_t *pa
   if (((uintptr_t)d_edge_list & 15) || ((uintptr_t)d_edge_indices & 7)) return fail("device arrays must be 16/8-byte aligned");
   CK(cudaSetDevice(c->device));
   TRY(set_graph(c, nv_global, parts, lnv, lne));
-  c->f32 = false;
-  c->d_rowptr64 = reinterpret_cast<const long long *>(d_edge_indices);
-  c->d_edges = reinterpret_cast<const Edge16 *>(d_edge_list);
-  c->d_tails32 = nullptr;
-  c->h2d_bytes = 0;
-  c->h2d_s = 0.0;
+  set_source(c, reinterpret_cast<const long long *>(d_edge_indices), reinterpret_cast<const Edge16 *>(d_edge_list), nullptr, false, 0.0, 0);
   return 0;
 }
 
@@ -1723,11 +1741,7 @@ int mvgpu_generate_rgg_shard_ex(mvgpu_ctx *c, int64_t nv_global, int unit_weight
   k_rgg_points<<<grid_for(P.n, 256, nsm), 256, 0, s>>>(P, X.p, UY.p);
   CK(cudaMemsetAsync(cnt.p, 0, sizeof(unsigned int) * (ncells + 1), s));
   k_rgg_bin<<<grid_for(P.n, 256, nsm), 256, 0, s>>>(P, X.p, UY.p, 0, cnt.p, nullptr, nullptr, nullptr, nullptr);
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.p, cstart.p, (int)(ncells + 1), s);
-  TRY(c->cub_tmp.ensure(tb));
-  tb = c->cub_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, cnt.p, cstart.p, (int)(ncells + 1), s));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, cnt.p, cstart.p, (int)(ncells + 1), s); }));
   unsigned int ncand = 0;
   CK(cudaMemcpyAsync(&ncand, cstart.p + ncells, sizeof ncand, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
@@ -1737,11 +1751,7 @@ int mvgpu_generate_rgg_shard_ex(mvgpu_ctx *c, int64_t nv_global, int unit_weight
   CK(cudaMemsetAsync(deg.p + P.n, 0, sizeof(long long), s));
   k_rgg_neighbours<false><<<grid_for(P.n, 128, nsm, 16), 128, 0, s>>>(P, X.p, UY.p, cstart.p, cx.p, cy.p, cgid.p, unit_weight, deg.p, nullptr);
   TRY(c->gen_rowptr.ensure(P.n + 1));
-  tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, deg.p, c->gen_rowptr.p, (int)(P.n + 1), s);
-  TRY(c->cub_tmp.ensure(tb));
-  tb = c->cub_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tb, deg.p, c->gen_rowptr.p, (int)(P.n + 1), s));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, deg.p, c->gen_rowptr.p, (int)(P.n + 1), s); }));
   long long lne = 0;
   CK(cudaMemcpyAsync(&lne, c->gen_rowptr.p + P.n, sizeof lne, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
@@ -1755,12 +1765,7 @@ int mvgpu_generate_rgg_shard_ex(mvgpu_ctx *c, int64_t nv_global, int unit_weight
   std::vector<int64_t> parts(p + 1);
   for (int q = 0; q <= p; q++) parts[q] = (nv_global * q) / p;
   TRY(set_graph(c, nv_global, parts.data(), P.n, lne));
-  c->f32 = false;
-  c->d_rowptr64 = c->gen_rowptr.p;
-  c->d_edges = c->gen_edges.p;
-  c->d_tails32 = nullptr;
-  c->h2d_bytes = 0;
-  c->h2d_s = 0.0;
+  set_source(c, c->gen_rowptr.p, c->gen_edges.p, nullptr, false, 0.0, 0);
   if (lne_out) *lne_out = lne;
   return 0;
 }
@@ -1784,13 +1789,9 @@ int mvgpu_set_initial_communities(mvgpu_ctx *c, const int64_t *comm) {
   if (!c) return fail("null argument");
   if (!comm) { c->have_init = false; return 0; }
   if (!c->have_graph) return fail("mvgpu_set_initial_communities: no shard yet (upload, attach or generate one first)");
-  std::vector<int32_t> h((size_t)c->lnv);
-  for (long long i = 0; i < c->lnv; i++) {
-    if (comm[i] < 0 || comm[i] >= c->nv_global)
-      return fail("mvgpu_set_initial_communities: community id " + std::to_string((long long)comm[i]) + " of local vertex " +
-                  std::to_string(i) + " outside [0, nv)");
-    h[i] = (int32_t)comm[i];
-  }
+  std::vector<int32_t> h;
+  const std::string err = narrow_ids(c, comm, "mvgpu_set_initial_communities", h);
+  if (!err.empty()) return fail(err);
   CK(cudaSetDevice(c->device));
   TRY(c->init_comm.ensure(c->lnv));
   if (c->lnv) CK(cudaMemcpy(c->init_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice));
@@ -1961,13 +1962,13 @@ int mv_layout_readback(mvgpu_ctx *c, int64_t *info16, uint32_t *rowptr, int32_t 
   if (!c) return fail("null ctx");
   if (!c->d_final) return fail("no run yet");
   if (info16) {
-    const int64_t v[16] = {c->lay_want, c->relabel, c->reordered ? 1 : 0, c->lay_stride, c->lay_nregions, c->lay_span[0],
-                           c->lay_span[1], c->lay_unordered, c->lay_has_self, c->simple_sorted ? 1 : 0,
-                           c->lay_first_ran ? 1 : 0, c->unit ? 1 : 0, c->roff.empty() ? 0 : c->roff[c->rank], c->nghost,
+    const int64_t v[16] = {c->lay.want, c->relabel, c->reordered ? 1 : 0, c->lay.stride, c->lay.nregions, c->lay.span[0],
+                           c->lay.span[1], c->lay.unordered, c->lay.has_self, c->simple_sorted ? 1 : 0,
+                           c->lay.first_ran ? 1 : 0, c->unit ? 1 : 0, c->roff.empty() ? 0 : c->roff[c->rank], c->nghost,
                            c->lnv, c->lne};
     memcpy(info16, v, sizeof v);
   }
-  const bool has_bfs = c->lay_want && c->relabel && c->lnv > 0, has_perm = c->relabel && c->lnv > 0;
+  const bool has_bfs = c->lay.want && c->relabel && c->lnv > 0, has_perm = c->relabel && c->lnv > 0;
   if ((bfs_key && !has_bfs) || ((perm || inv || lab) && !has_perm) || ((rowptr2 || tails2) && !c->reordered) ||
       (weights2 && (!c->reordered || c->unit)))
     return fail("mv_layout_readback: the last run did not build that array");
@@ -1975,7 +1976,7 @@ int mv_layout_readback(mvgpu_ctx *c, int64_t *info16, uint32_t *rowptr, int32_t 
   cudaStream_t s = c->stream;
   const size_t nv = (size_t)c->lnv, ne = (size_t)c->lne;
   if (rowptr) CK(cudaMemcpyAsync(rowptr, c->rowptr.p, sizeof(uint32_t) * (nv + 1), cudaMemcpyDeviceToHost, s));
-  if (tails && ne) CK(cudaMemcpyAsync(tails, c->lay_tails, sizeof(int32_t) * ne, cudaMemcpyDeviceToHost, s));
+  if (tails && ne) CK(cudaMemcpyAsync(tails, c->lay.tails, sizeof(int32_t) * ne, cudaMemcpyDeviceToHost, s));
   if (bfs_key) CK(cudaMemcpyAsync(bfs_key, c->bfs_key.p, sizeof(uint32_t) * nv, cudaMemcpyDeviceToHost, s));
   if (perm) CK(cudaMemcpyAsync(perm, c->perm.p, sizeof(int32_t) * nv, cudaMemcpyDeviceToHost, s));
   if (inv) CK(cudaMemcpyAsync(inv, c->inv.p, sizeof(int32_t) * nv, cudaMemcpyDeviceToHost, s));
@@ -1994,7 +1995,6 @@ int mvgpu_upload_shard32(mvgpu_ctx *c, int32_t nv_global, const int32_t *parts, 
   CK(cudaSetDevice(c->device));
   std::vector<int64_t> parts64(parts, parts + c->nranks + 1);
   TRY(set_graph(c, nv_global, parts64.data(), lnv, lne));
-  c->f32 = true;
   DevBuf<Edge8> e8;
   DevBuf<int32_t> rp32;
   TRY(e8.ensure((size_t)lne)); TRY(rp32.ensure((size_t)lnv + 1));
@@ -2009,11 +2009,8 @@ int mvgpu_upload_shard32(mvgpu_ctx *c, int32_t nv_global, const int32_t *parts, 
   CK(cudaEventSynchronize(b));
   float ms = 0;
   CK(cudaEventElapsedTime(&ms, a, b));
-  c->h2d_s = ms * 1e-3;
-  c->h2d_bytes = (long long)sizeof(int32_t) * (lnv + 1) + (long long)sizeof(Edge8) * lne;
-  c->d_rowptr64 = c->in_rowptr.p;
-  c->d_edges = c->in_edges.p;
-  c->d_tails32 = nullptr;
+  set_source(c, c->in_rowptr.p, c->in_edges.p, nullptr, true, ms * 1e-3,
+             (long long)sizeof(int32_t) * (lnv + 1) + (long long)sizeof(Edge8) * lne);
   return 0;
 }
 
