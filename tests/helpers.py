@@ -251,3 +251,83 @@ def rmat_graph(scale, edge_factor, seed, a=0.57, b=0.19, c=0.19, dyadic=False):
     edges["tail"] = d2
     edges["weight"] = w2
     return n, rowptr, edges
+
+
+# ---- rounding witnesses: graphs whose first decision depends on the order of one fp64 sum (tests/golden/make_golden_rounding.py)
+
+WITNESS_NV, WITNESS_V = 64, 40          # the witness vertex sits in the aligned group [32, 64) and on rank 1 of 2 / 2 of 4
+WITNESS_B, WITNESS_A, WITNESS_U = 10, 11, 12
+
+
+def rounding_witness(name):
+    """(nv, rowptr, edges, X) of a witness graph; X is the starting assignment (None: singletons).
+
+    R1 ("r1_ck1", "r1_ck2", "r1_subrange"): vertex v has three parallel edges to A of weights 0.1, 0.2, 0.3 and two to
+    B of weights 0.5, 0.1, interleaved with three light edges; k_A == k_B bitwise (both 0.6.. + 10 = 10.6) and
+    B < A < v, so the gains of A and B differ only in their counter sums.  In edge order A's sum is 0.6000000000000001
+    and A wins; summed in reverse (0.6) the gains tie and the smaller id B wins.  ck1 lists A first (the first
+    community of pass 1), ck2 lists B first (A is the second community found); subrange adds a dense block around v so
+    that its 32-vertex group holds more edges than one staging buffer.
+    R2 ("r2_own"): X puts v with u (three parallel edges 0.1, 0.2, 0.3, interleaved); the candidate B has one edge of
+    weight 0.6000000000000001 and a_B == a_X - k_v bitwise, so the gain of B is 2 (0.6000000000000001 - counter[0]):
+    0 in edge order (v stays), positive with counter[0] summed in reverse (v moves)."""
+    nv, v = WITNESS_NV, WITNESS_V
+    rng = np.random.default_rng(2024)
+    adj = [[] for _ in range(nv)]
+
+    def edge(a, b, w):
+        adj[a].append((b, w))
+        adj[b].append((a, w))
+
+    light = [50, 51, 52]
+    if name.startswith("r1"):
+        A, B = WITNESS_A, WITNESS_B
+        if name == "r1_ck2":
+            order = [(B, 0.5), (A, 0.1), (light[0], 0.01), (A, 0.2), (B, 0.1), (light[1], 0.01), (A, 0.3),
+                     (light[2], 0.01)]
+        else:
+            order = [(A, 0.1), (light[0], 0.01), (B, 0.5), (A, 0.2), (light[1], 0.01), (A, 0.3), (B, 0.1),
+                     (light[2], 0.01)]
+        pend = {A: 20, B: 21}
+    elif name == "r2_own":
+        u, B = WITNESS_U, WITNESS_B
+        order = [(u, 0.1), (light[0], 0.01), (u, 0.2), (B, 0.6000000000000001), (u, 0.3), (light[1], 0.01)]
+        pend = {u: 20, B: 21}
+    else:
+        raise ValueError(name)
+    for t, w in order:                          # v's list in this order; each tail's list gets the edge in this order too
+        edge(v, t, w)
+    for t, p in pend.items():
+        edge(t, p, 10.0)
+    special = {v, *pend, *pend.values(), *light}
+    others = [x for x in range(nv) if x not in special]
+    for x in others:                            # sparse background, general weights
+        for y in rng.choice(others, 3, replace=False):
+            if y != x:
+                edge(x, int(y), float(rng.uniform(0.5, 1.5)))
+    for x in light:
+        edge(x, int(rng.choice(others)), float(rng.uniform(0.5, 1.5)))
+    if name == "r1_subrange":
+        block = [x for x in range(32, 64) if x not in special]
+        for i, x in enumerate(block):
+            for y in block[i + 1:]:
+                if rng.random() < 0.6:
+                    edge(x, y, float(rng.uniform(0.5, 1.5)))
+    rowptr = np.zeros(nv + 1, np.int64)
+    rowptr[1:] = np.cumsum([len(a) for a in adj])
+    edges = np.zeros(int(rowptr[-1]), hg.EDGE_DTYPE)
+    edges["tail"] = [t for a in adj for t, _ in a]
+    edges["weight"] = [w for a in adj for _, w in a]
+    X = None
+    if name == "r2_own":
+        X = np.arange(nv, dtype=np.int64)
+        X[v] = WITNESS_U
+    return nv, rowptr, edges, X
+
+
+def reversed_adjacency(rowptr, edges, v):
+    """The same graph with vertex v's adjacency list in reverse order."""
+    e = edges.copy()
+    a, b = int(rowptr[v]), int(rowptr[v + 1])
+    e[a:b] = edges[a:b][::-1]
+    return e

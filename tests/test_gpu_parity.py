@@ -2,7 +2,8 @@
 against the golden traces of the unmodified reference and against the C oracle on the same inputs.
 Bar: bit-exact community ids, iteration counts, moved counts and modularity for unit weights and for dyadic weights
 (k * 2^-j: every sum exact); |dQ| <= 1e-6 (BASELINE.json north_star tolerance) for the Euclidean weights of the -w RGGs,
-whose sums depend on the order of the additions."""
+whose sums depend on the order of the additions.  Those weights are pinned one step at a time, per vertex, in
+tests/test_gpu_weighted_step.py."""
 import numpy as np
 import pytest
 
