@@ -96,6 +96,21 @@ int mvgpu_generate_rgg_shard_ex(mvgpu_ctx *ctx, int64_t nv_global, int unit_weig
                                 int64_t *lne_out);
 /* Copy the shard's reference-format arrays (lnv+1 offsets, lne 16-byte records) back to the host. */
 int mvgpu_download_shard(mvgpu_ctx *ctx, int64_t *edge_indices, void *edge_list);
+/* Change the shard in place on the device (DESIGN.md §3.11): n_del deletions (del_src[i], del_dst[i]) and n_ins
+ * insertions (ins_src[i], ins_dst[i], ins_weight[i]), host arrays in global ids, src owned by this rank.  Per row:
+ * every old record whose tail is the dst of a deletion of that row is dropped (parallel records included; deletions
+ * match old records only, so delete + insert of one pair replaces its weight); the insertions, stably sorted by dst,
+ * are merged into the surviving records by "next old record while its tail <= the next insertion's dst, else the
+ * insertion" (std::stable_sort of the concatenation for rows sorted by tail).  Both directions of an undirected edge
+ * are the caller's to give.  Validated before anything changes: src in [base, bound), dst in [0, nv), the new lne
+ * < 2^32, and the shard's edge_indices (0 first, lne last, never decreasing); refused for a compact-format or 32-bit
+ * shard.  Synchronous; collective when nranks > 1 (every rank calls
+ * it, with an empty batch if it has none), and one rank's failure fails every rank with all shards unchanged.
+ * After success: *lne_out (may be NULL) = the new lne; the shard lives in library memory (an attached shard's arrays
+ * are never written); the initial assignment is kept, mvgpu_get_communities still returns the last run's result, a
+ * NULL evaluation and the per-community getters wait for the next run or evaluation; h2d figures are 0. */
+int mvgpu_update_shard(mvgpu_ctx *ctx, int64_t n_del, const int64_t *del_src, const int64_t *del_dst, int64_t n_ins,
+                       const int64_t *ins_src, const int64_t *ins_dst, const double *ins_weight, int64_t *lne_out);
 
 /* ---- the Louvain phase (dspl.hpp:1280-1441) --------------------------------------------------- */
 /* lower/thresh as in the reference (main.cpp:149,70); *iters counts the rejected last iteration

@@ -34,6 +34,7 @@
 #include "scan_queue.cuh"
 #include "nccl_dyn.h"
 #include "rgg_gpu.cuh"
+#include "merge_gpu.cuh"
 
 // host-only helper of the compact upload (narrow.cpp): 16-byte edge records -> 4-byte tails + validation
 extern "C" void mv_narrow_edges(const void *edge_records, long long n, long long nv, long long base, long long bound,
@@ -73,6 +74,7 @@ struct DevBuf {              // grow-only device buffer (allocations are cached 
   DevBuf(const DevBuf &) = delete;
   DevBuf &operator=(const DevBuf &) = delete;
   ~DevBuf() { release(); }
+  void swap(DevBuf &o) { std::swap(p, o.p); std::swap(cap, o.cap); gen++; o.gen++; }
   int ensure(size_t n) {
     if (n <= cap && p) return 0;
     if (p) cudaFree(p);
@@ -1345,6 +1347,86 @@ int evaluate(mvgpu_ctx *c, const int64_t *comm, mvgpu_quality *out, const char *
   return rc;
 }
 
+// ---- shard update (DESIGN.md §3.11, merge_gpu.cuh) -------------------------------------------------------------------
+// The shard (n rows, rowptr/edges, lne records) with the sorted deletion keys dkey and the stably sorted insertion keys
+// ikey merged in (iidx: batch index of each sorted insertion, iw: weights in batch order) -> nrow / nedges, *lne_out.
+// Reads the old shard only.  Fails (writing nothing but the outputs) when the result would hold 2^32 records or more.
+int merge_records(mvgpu_ctx *c, long long n, const long long *rowptr, const Edge16 *edges, long long lne,
+                  const unsigned long long *dkey, long long ndel, const unsigned long long *ikey, const unsigned int *iidx,
+                  const double *iw, long long nins, DevBuf<long long> &nrow, DevBuf<Edge16> &nedges, long long *lne_out) {
+  cudaStream_t s = c->stream;
+  const int nsm = c->num_sms;
+  DevBuf<unsigned int> dstart, istart, kept, kscan;
+  DevBuf<int32_t> erow;
+  DevBuf<long long> mval, mscan, deg;
+  TRY(dstart.ensure(n + 1)); TRY(istart.ensure(n + 1));
+  TRY(kept.ensure(lne + 1)); TRY(kscan.ensure(lne + 1));
+  TRY(deg.ensure(n + 1)); TRY(nrow.ensure(n + 1));
+  k_row_bounds<<<grid_for(n + 1, 256, nsm), 256, 0, s>>>(dkey, ndel, n, dstart.p);
+  k_row_bounds<<<grid_for(n + 1, 256, nsm), 256, 0, s>>>(ikey, nins, n, istart.p);
+  CK(cudaMemsetAsync(kept.p + lne, 0, sizeof(unsigned int), s));
+  if (lne) {
+    TRY(erow.ensure(lne)); TRY(mval.ensure(lne)); TRY(mscan.ensure(lne));
+    k_merge_keep<<<grid_for(lne, 256, nsm, 16), 256, 0, s>>>(rowptr, edges, lne, n, dkey, dstart.p, erow.p, kept.p, mval.p);
+    TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::InclusiveScanByKey(t, tb, erow.p, mval.p, mscan.p, MaxLL(), lne, cub::Equality(), s); }));
+  }
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, kept.p, kscan.p, lne + 1, s); }));
+  k_merge_degree<<<grid_for(n + 1, 256, nsm), 256, 0, s>>>(rowptr, kscan.p, istart.p, n, deg.p);
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, deg.p, nrow.p, n + 1, s); }));
+  long long lne2 = 0;
+  CK(cudaMemcpyAsync(&lne2, nrow.p + n, sizeof lne2, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (lne2 >= (1LL << 32)) return fail("the updated shard would hold lne >= 2^32 records (32-bit edge offsets would overflow)");
+  TRY(nedges.ensure(lne2));
+  if (lne) k_merge_old<<<grid_for(lne, 256, nsm, 16), 256, 0, s>>>(rowptr, edges, lne, erow.p, kscan.p, mscan.p, ikey, istart.p, nrow.p, nedges.p);
+  if (nins) k_merge_ins<<<grid_for(nins, 256, nsm, 16), 256, 0, s>>>(ikey, iidx, iw, nins, istart.p, rowptr, kscan.p, mscan.p, nrow.p, nedges.p);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(s));
+  *lne_out = lne2;
+  return 0;
+}
+
+// This rank's part of mvgpu_update_shard before the agreement: the batch to the device, validated, sorted and merged
+// into nrow / nedges.  Leaves the shard itself as it is.
+int update_prepare(mvgpu_ctx *c, long long n_del, const int64_t *del_src, const int64_t *del_dst, long long n_ins,
+                   const int64_t *ins_src, const int64_t *ins_dst, const double *ins_weight, DevBuf<long long> &nrow,
+                   DevBuf<Edge16> &nedges, long long *lne_out) {
+  cudaStream_t s = c->stream;
+  const int nsm = c->num_sms;
+  DevBuf<long long> dsrc, ddst, isrc, idst;
+  DevBuf<double> iw;
+  DevBuf<unsigned long long> dkey, dkey_s, ikey, ikey_s;
+  DevBuf<unsigned int> iidx, iidx_s, bad;
+  TRY(dsrc.ensure(n_del)); TRY(ddst.ensure(n_del)); TRY(dkey.ensure(n_del)); TRY(dkey_s.ensure(n_del));
+  TRY(isrc.ensure(n_ins)); TRY(idst.ensure(n_ins)); TRY(iw.ensure(n_ins)); TRY(ikey.ensure(n_ins)); TRY(ikey_s.ensure(n_ins));
+  TRY(iidx.ensure(n_ins)); TRY(iidx_s.ensure(n_ins)); TRY(bad.ensure(1));
+  if (n_del) {
+    CK(cudaMemcpyAsync(dsrc.p, del_src, sizeof(long long) * n_del, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ddst.p, del_dst, sizeof(long long) * n_del, cudaMemcpyHostToDevice, s));
+  }
+  if (n_ins) {
+    CK(cudaMemcpyAsync(isrc.p, ins_src, sizeof(long long) * n_ins, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(idst.p, ins_dst, sizeof(long long) * n_ins, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(iw.p, ins_weight, sizeof(double) * n_ins, cudaMemcpyHostToDevice, s));
+  }
+  CK(cudaMemsetAsync(bad.p, 0, sizeof(unsigned int), s));
+  k_rowptr_check<<<grid_for(c->lnv + 1, 256, nsm), 256, 0, s>>>(c->d_rowptr64, c->lnv, c->lne, bad.p);
+  if (n_del) k_batch_keys<<<grid_for(n_del, 256, nsm), 256, 0, s>>>(dsrc.p, ddst.p, n_del, c->base, c->bound, c->nv_global, dkey.p, nullptr, bad.p);
+  if (n_ins) k_batch_keys<<<grid_for(n_ins, 256, nsm), 256, 0, s>>>(isrc.p, idst.p, n_ins, c->base, c->bound, c->nv_global, ikey.p, iidx.p, bad.p);
+  CK(cudaGetLastError());
+  unsigned int hbad = 0;
+  CK(cudaMemcpyAsync(&hbad, bad.p, sizeof hbad, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (hbad & kBadRowptr) return fail("mvgpu_update_shard: edge_indices malformed (must start at 0, end at lne and never decrease)");
+  if (hbad & kBadBatch) return fail("mvgpu_update_shard: a batch record lies outside the shard (src must be in [base, bound), dst in [0, nv))");
+  dsrc.release(); ddst.release(); isrc.release(); idst.release();
+  // keys are (local row < 2^31) << 31 | (tail < 2^31): 62 bits; the radix sort is stable, so equal insertion keys keep
+  // batch order
+  if (n_del) TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortKeys(t, tb, dkey.p, dkey_s.p, (int)n_del, 0, 62, s); }));
+  if (n_ins) TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, ikey.p, ikey_s.p, iidx.p, iidx_s.p, (int)n_ins, 0, 62, s); }));
+  return merge_records(c, c->lnv, c->d_rowptr64, c->d_edges, c->lne, dkey_s.p, n_del, ikey_s.p, iidx_s.p, iw.p, n_ins, nrow, nedges, lne_out);
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -1375,7 +1457,7 @@ static int add_random_edges(mvgpu_ctx *c, const RggParams &P, int64_t nv, int un
   DevBuf<long long> dsoff, nrow;
   DevBuf<int> di, dgj;
   DevBuf<unsigned long long> key, skey, xkey, sxkey;
-  DevBuf<unsigned int> qidx, sq, emit, epos, xidx, sxidx, add, xstart;
+  DevBuf<unsigned int> qidx, sq, emit, epos, xidx, sxidx;
   DevBuf<double> xw;
   TRY(dsoff.ensure(p + 1)); TRY(di.ensure(nrande)); TRY(dgj.ensure(nrande));
   TRY(key.ensure(nrande)); TRY(skey.ensure(nrande)); TRY(qidx.ensure(nrande)); TRY(sq.ensure(nrande));
@@ -1392,22 +1474,15 @@ static int add_random_edges(mvgpu_ctx *c, const RggParams &P, int64_t nv, int un
   CK(cudaStreamSynchronize(s));
   if (!nextra) return 0;
   TRY(xkey.ensure(nextra)); TRY(sxkey.ensure(nextra)); TRY(xidx.ensure(nextra)); TRY(sxidx.ensure(nextra)); TRY(xw.ensure(nextra));
-  TRY(add.ensure(P.n + 1)); TRY(xstart.ensure(P.n + 1)); TRY(nrow.ensure(P.n + 1));
-  CK(cudaMemsetAsync(add.p, 0, sizeof(unsigned int) * (P.n + 1), s));
   k_rande_emit<<<grid_for(nrande, 256, nsm), 256, 0, s>>>(R, P, dsoff.p, di.p, dgj.p, nrande, emit.p, epos.p, unit, X3, Y3, xkey.p, xw.p,
-                                                        xidx.p, add.p);
+                                                        xidx.p);
   TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, xkey.p, sxkey.p, xidx.p, sxidx.p, (int)nextra, 0, 62, s); }));
-  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, add.p, xstart.p, (int)(P.n + 1), s); }));
-  k_rande_rowptr<<<grid_for(P.n + 1, 256, nsm), 256, 0, s>>>(c->gen_rowptr.p, xstart.p, P.n, nrow.p);
-  const long long lne2 = *lne_io + (long long)nextra;
+  // the extras are an insert-only batch in push order: merged like an update, RGG records first among equal tails
   DevBuf<Edge16> merged;
-  TRY(merged.ensure(lne2));
-  k_rande_merge<<<grid_for(P.n, 256, nsm, 16), 256, 0, s>>>(c->gen_rowptr.p, c->gen_edges.p, xstart.p, sxkey.p, sxidx.p, xw.p, P.n, nrow.p,
-                                                          merged.p);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(s));
-  std::swap(c->gen_edges.p, merged.p); std::swap(c->gen_edges.cap, merged.cap); c->gen_edges.gen++;
-  std::swap(c->gen_rowptr.p, nrow.p); std::swap(c->gen_rowptr.cap, nrow.cap); c->gen_rowptr.gen++;
+  long long lne2 = 0;
+  TRY(merge_records(c, P.n, c->gen_rowptr.p, c->gen_edges.p, *lne_io, nullptr, 0, sxkey.p, sxidx.p, xw.p, nextra, nrow, merged, &lne2));
+  c->gen_edges.swap(merged);
+  c->gen_rowptr.swap(nrow);
   *lne_io = lne2;
   return 0;
 }
@@ -1777,6 +1852,48 @@ int mvgpu_download_shard(mvgpu_ctx *c, int64_t *edge_indices, void *edge_list) {
   if (edge_indices) CK(cudaMemcpyAsync(edge_indices, c->d_rowptr64, sizeof(long long) * (c->lnv + 1), cudaMemcpyDeviceToHost, c->stream));
   if (edge_list && c->lne) CK(cudaMemcpyAsync(edge_list, c->d_edges, sizeof(Edge16) * c->lne, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+int mvgpu_update_shard(mvgpu_ctx *c, int64_t n_del, const int64_t *del_src, const int64_t *del_dst, int64_t n_ins,
+                       const int64_t *ins_src, const int64_t *ins_dst, const double *ins_weight, int64_t *lne_out) {
+  if (!c) return fail("null ctx");
+  CK(cudaSetDevice(c->device));
+  if (c->nranks > 1 && !c->comm && !c->hc.is_open()) return fail("mvgpu_update_shard is collective on several ranks: call mvgpu_comm_init first");
+  // every local finding waits for the agreement below, so that one rank's bad batch fails every rank
+  std::string err;
+  if (!c->have_graph || !c->d_rowptr64) err = "no shard on the device";
+  else if (c->d_tails32) err = "the shard was uploaded in the compact format: it has no records to update";
+  else if (c->f32) err = "a shard uploaded with mvgpu_upload_shard32 cannot be updated";
+  else if (n_del < 0 || n_ins < 0) err = "negative batch size";
+  else if (n_del >= (1LL << 31) || n_ins >= (1LL << 31)) err = "batch too large: fewer than 2^31 deletions and 2^31 insertions per call";
+  else if ((n_del && (!del_src || !del_dst)) || (n_ins && (!ins_src || !ins_dst || !ins_weight))) err = "null batch array";
+  if (!err.empty()) err = "mvgpu_update_shard: " + err;
+  DevBuf<long long> nrow;
+  DevBuf<Edge16> nedges;
+  long long lne2 = 0;
+  if (err.empty() && update_prepare(c, n_del, del_src, del_dst, n_ins, ins_src, ins_dst, ins_weight, nrow, nedges, &lne2)) err = g_err;
+  if (c->nranks > 1) {
+    TRY(c->scratch.ensure(sizeof(Scalars)));
+    long long any = err.empty() ? 0 : 1;
+    TRY(coll_allreduce_i64(c, &any, 1, false));
+    if (any && err.empty()) err = "mvgpu_update_shard: another rank rejected its batch";
+  }
+  if (!err.empty()) return fail(err);
+  // the last run's assignment is resolved while its arrays still describe it: communities() keeps returning it
+  if (c->run_on_shard) TRY(final_in_caller_order(c));
+  // the result lives in library buffers from now on (never in an attached shard's arrays): the generator's, if the
+  // shard came from there, the upload buffers otherwise; the old arrays go with nrow / nedges
+  const bool gen = c->d_edges == c->gen_edges.p;
+  DevBuf<long long> &rp = gen ? c->gen_rowptr : c->in_rowptr;
+  DevBuf<Edge16> &ed = gen ? c->gen_edges : c->in_edges;
+  rp.swap(nrow);
+  ed.swap(nedges);
+  c->lne = lne2;
+  set_source(c, rp.p, ed.p, nullptr, false, 0.0, 0);
+  c->run_on_shard = c->eval_on_shard = false;   // the initial assignment stays: parts and lnv have not changed
+  c->peers_ready = false;                       // ghost lists and receive offsets change with the records, on every rank
+  if (lne_out) *lne_out = lne2;
   return 0;
 }
 

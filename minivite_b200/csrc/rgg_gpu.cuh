@@ -252,7 +252,7 @@ __global__ void __launch_bounds__(256) k_rande_first(const unsigned long long *s
 __global__ void __launch_bounds__(256) k_rande_emit(RandeParams rp, RggParams gp, const long long *soff, const int *di, const int *dgj,
                                                     long long nr, const unsigned int *emit, const unsigned int *epos, int unit,
                                                     const double *X3, const double *Y3, unsigned long long *xkey, double *xw,
-                                                    unsigned int *xidx, unsigned int *add) {
+                                                    unsigned int *xidx) {
   const int s0 = max(0, rp.me - 1);
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < nr; q += (long long)gridDim.x * blockDim.x) {
     const unsigned int cnt = emit[q];
@@ -279,42 +279,11 @@ __global__ void __launch_bounds__(256) k_rande_emit(RandeParams rp, RggParams gp
     if (s == rp.me) {
       xkey[e] = ((unsigned long long)i << 31) | (unsigned long long)gj;
       xw[e] = w; xidx[e] = e;
-      atomicAdd(&add[i], 1u);
       e++;
     }
     if (target == rp.me) {
       xkey[e] = ((unsigned long long)j << 31) | (unsigned long long)gi;
       xw[e] = w; xidx[e] = e;
-      atomicAdd(&add[j], 1u);
-    }
-  }
-}
-
-__global__ void __launch_bounds__(256) k_rande_rowptr(const long long *rowptr, const unsigned int *xstart, long long n, long long *nrow) {
-  for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v <= n; v += (long long)gridDim.x * blockDim.x)
-    nrow[v] = rowptr[v] + (long long)xstart[v];
-}
-
-// per vertex: RGG list and extras (both ascending by tail) merged, RGG entries first among equal tails, extras in
-// push order among themselves (= std::stable_sort of the concatenation)
-__global__ void __launch_bounds__(256) k_rande_merge(const long long *rowptr, const Edge16 *edges, const unsigned int *xstart,
-                                                     const unsigned long long *sxkey, const unsigned int *sxidx, const double *xw,
-                                                     long long n, const long long *nrow, Edge16 *out) {
-  for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < n; v += (long long)gridDim.x * blockDim.x) {
-    long long a = rowptr[v];
-    const long long ae = rowptr[v + 1];
-    unsigned int b = xstart[v];
-    const unsigned int be = xstart[v + 1];
-    Edge16 *o = out + nrow[v];
-    while (a < ae || b < be) {
-      bool take_a = b >= be;
-      long long bt = 0;
-      if (!take_a) {
-        bt = (long long)(sxkey[b] & 0x7fffffffULL);
-        take_a = a < ae && edges[a].tail <= bt;
-      }
-      if (take_a) *o++ = edges[a++];
-      else { Edge16 r; r.tail = bt; r.weight = xw[sxidx[b]]; *o++ = r; b++; }
     }
   }
 }

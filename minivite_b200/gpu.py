@@ -41,7 +41,7 @@ EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_dest
            "mvgpu_get_communities", "mvgpu_get_communities_device", "mvgpu_upload_shard32", "mvgpu_louvain32", "mvgpu_get_communities32", "mvgpu_set_option", "mvgpu_get_trace",
            "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method",
            "mvgpu_set_initial_communities", "mvgpu_get_converged", "mvgpu_evaluate_communities",
-           "mvgpu_get_community_stats", "mvgpu_get_compact_communities"]
+           "mvgpu_get_community_stats", "mvgpu_get_compact_communities", "mvgpu_update_shard"]
 
 _lib = None
 
@@ -65,6 +65,7 @@ def lib():
         L.mvgpu_generate_rgg_shard.argtypes = [vp, i64, ci, ctypes.POINTER(i64)]
         L.mvgpu_generate_rgg_shard_ex.argtypes = [vp, i64, ci, ci, ctypes.c_double, ctypes.POINTER(i64)]
         L.mvgpu_download_shard.argtypes = [vp, vp, vp]
+        L.mvgpu_update_shard.argtypes = [vp, i64, vp, vp, i64, vp, vp, vp, ctypes.POINTER(i64)]
         L.mvgpu_louvain.argtypes = [vp, dbl, dbl, ctypes.POINTER(ci), ctypes.POINTER(dbl)]
         L.mvgpu_get_communities.argtypes = [vp, vp]
         L.mvgpu_set_initial_communities.argtypes = [vp, vp]
@@ -185,6 +186,31 @@ class LouvainGPU:
         edges = np.zeros(info["lne"], dtype=np.dtype([("tail", "<i8"), ("weight", "<f8")]))
         _ck(lib().mvgpu_download_shard(self._h, rowptr.ctypes.data, edges.ctypes.data if info["lne"] else None))
         return rowptr, edges
+
+    def update_shard(self, delete=None, insert=None):
+        """Change the shard in place on the device (DESIGN.md §3.11): delete=(src, dst) drops every record (src, dst) of
+        the shard, insert=(src, dst, w) merges new records in; global ids, src owned by this rank, both directions of an
+        undirected edge given by the caller.  Collective with several ranks (pass None, None when a rank has no
+        changes).  Returns the new lne."""
+        def cols(t, dtypes, what):
+            if t is None:
+                return [np.zeros(0, d) for d in dtypes]
+            if len(t) != len(dtypes):
+                raise ValueError(f"{what} takes {len(dtypes)} arrays")
+            out = [np.ascontiguousarray(a, dtype=d).reshape(-1) for a, d in zip(t, dtypes)]
+            if any(a.size != out[0].size for a in out):
+                raise ValueError(f"{what}: arrays of different lengths")
+            return out
+        ds, dd = cols(delete, (np.int64, np.int64), "delete")
+        is_, id_, iw = cols(insert, (np.int64, np.int64, np.float64), "insert")
+
+        def ptr(a):
+            return a.ctypes.data if a.size else None
+        lne = ctypes.c_int64(0)
+        _ck(lib().mvgpu_update_shard(self._h, ds.size, ptr(ds), ptr(dd), is_.size, ptr(is_), ptr(id_), ptr(iw),
+                                     ctypes.byref(lne)))
+        self._keep = None            # an attached shard's arrays are no longer read
+        return lne.value
 
     def set_option(self, name, value):
         _ck(lib().mvgpu_set_option(self._h, name.encode(), int(value)))
