@@ -156,6 +156,27 @@ int mvgpu_get_community_stats(mvgpu_ctx *ctx, int64_t *size, double *volume, dou
  * ascending caller id, in [0, communities); independent of the rank count and of the locality renumbering. */
 int mvgpu_get_compact_communities(mvgpu_ctx *ctx, int64_t *out);
 
+/* ---- splitting disconnected communities (DESIGN.md §3.12) ------------------------------------------------------------
+ * A Louvain phase can leave a community in several pieces: a vertex that joined through a bridge vertex stays after the
+ * bridge leaves.  Two vertices i, j are joined when X(i) = X(j) and the shard stores a record i->j or j->i (any weight,
+ * zero included; self loops join nothing; a record stored in one direction only joins too).  Y gives every vertex the
+ * smallest caller global id of its component under that relation: canonical (independent of the rank count, the
+ * renumbering and the device's order), a member of the community, so a valid input to mvgpu_set_initial_communities and
+ * mvgpu_evaluate_communities.  Splitting never lowers the modularity.  Every count is global and identical on every rank. */
+typedef struct {
+  int64_t communities;  /* non-empty communities of X */
+  int64_t components;   /* components, = the communities of Y */
+  int64_t disconnected; /* communities of X with more than one component */
+  int32_t rounds;       /* hook + pointer-jump rounds the device took */
+  double split_s;       /* device time of the call (CUDA events on the context's stream) */
+} mvgpu_split_report;
+/* Collective.  comm: lnv community ids in [0, nv) in the caller's vertex numbering; NULL splits the assignment the last
+ * mvgpu_louvain on this shard returned.  out: lnv entries of Y.  Errors as in mvgpu_evaluate_communities (a bad id on
+ * any rank, NULL without a run, ranks that disagree on NULL, a shard from mvgpu_upload_shard32) fail the call on every
+ * rank, and then nothing is written to out.  Leaves everything the last run reports and the initial assignment as they
+ * were; the per-community arrays of the last evaluation are gone (their getters fail until the next evaluation). */
+int mvgpu_split_communities(mvgpu_ctx *ctx, const int64_t *comm, int64_t *out, mvgpu_split_report *rep);
+
 /* currComm of this rank's vertices at exit (global community ids), lnv entries. */
 int mvgpu_get_communities(mvgpu_ctx *ctx, int64_t *out);
 /* Same values left in device memory (int32 global ids); valid until the next mvgpu_louvain. */

@@ -28,6 +28,9 @@ struct GpuRankContext {
   bool quality = false;                                // -q: evaluate the returned assignment after the run
   const std::vector<GraphElem> *eval_comm = nullptr;   // -E: evaluate this assignment instead of running the phase
   mvgpu_quality q{};                                   // -q / -E: the evaluation (global values)
+  bool split = false;                                  // -C: split the run's (or -E's) assignment into connected pieces
+  mvgpu_split_report split_rep{};                      // -C: the split's counts (global values)
+  std::vector<GraphElem> split_comm;                   // -C: the split assignment of this rank's vertices
 };
 
 [[noreturn]] inline void mv_abort(const std::string &where) {
@@ -66,16 +69,36 @@ inline void mv_apply_warm_start(mvgpu_ctx *ctx, const GpuRankContext &rc) {
   if (rc.init_comm && mvgpu_set_initial_communities(ctx, rc.init_comm->data())) mv_abort("mvgpu_set_initial_communities");
   if (rc.stop_after && mvgpu_set_option(ctx, "stop_after", rc.stop_after)) mv_abort("stop_after");
 }
-// -E: evaluate the given assignment and run no Louvain phase (true: done, the caller returns)
+// -C: split `comm` (NULL: the run's result) into rc.split_comm
+inline void mv_split(mvgpu_ctx *ctx, GpuRankContext &rc, const GraphElem *comm, GraphElem lnv) {
+  rc.split_comm.assign(lnv + 1, 0);                // never an empty array: the call takes a non-NULL out on every rank
+  if (mvgpu_split_communities(ctx, comm, rc.split_comm.data(), &rc.split_rep)) mv_abort("mvgpu_split_communities");
+  rc.split_comm.resize(lnv);
+}
+// -E: evaluate the given assignment (with -C: its split) and run no Louvain phase (true: done, the caller returns)
 inline bool mv_evaluate_only(mvgpu_ctx *ctx, GpuRankContext &rc) {
   if (!rc.eval_comm) return false;
-  if (mvgpu_evaluate_communities(ctx, rc.eval_comm->data(), &rc.q)) mv_abort("mvgpu_evaluate_communities");
+  const GraphElem *X = rc.eval_comm->data();
+  if (rc.split) {
+    mv_split(ctx, rc, X, (GraphElem)rc.eval_comm->size());
+    X = rc.split_comm.data();
+  }
+  if (mvgpu_evaluate_communities(ctx, X, &rc.q)) mv_abort("mvgpu_evaluate_communities");
   mvgpu_destroy(ctx);
   return true;
 }
-// -q: evaluate the assignment the run returned
-inline void mv_evaluate_run(mvgpu_ctx *ctx, GpuRankContext &rc) {
-  if (rc.quality && mvgpu_evaluate_communities(ctx, nullptr, &rc.q)) mv_abort("mvgpu_evaluate_communities");
+// -C: split the assignment the run returned; -q: evaluate the run's assignment (with -C: its split)
+inline void mv_evaluate_run(mvgpu_ctx *ctx, GpuRankContext &rc, GraphElem lnv) {
+  if (rc.split) mv_split(ctx, rc, nullptr, lnv);
+  if (rc.quality && mvgpu_evaluate_communities(ctx, rc.split ? rc.split_comm.data() : nullptr, &rc.q))
+    mv_abort("mvgpu_evaluate_communities");
+}
+// -o: the run's assignment (with -C: its split)
+inline void mv_result(mvgpu_ctx *ctx, GpuRankContext &rc, GraphElem lnv) {
+  if (!rc.comm_out) return;
+  if (rc.split) { *rc.comm_out = rc.split_comm; return; }
+  rc.comm_out->resize(lnv);
+  if (mvgpu_get_communities(ctx, rc.comm_out->data())) mv_abort("mvgpu_get_communities");
 }
 inline void mv_read_converged(mvgpu_ctx *ctx, GpuRankContext &rc) {
   int conv = 1;
@@ -118,7 +141,7 @@ inline GraphWeight distLouvainMethod(const int me, const int nprocs, const Graph
   double mod = 0.0;
   for (int rep = mv_env_repeat(); rep > 0; rep--)
     if (mvgpu_louvain(ctx, lower, thresh, &iters, &mod)) mv_abort("mvgpu_louvain");
-  mv_evaluate_run(ctx, rc);
+  mv_evaluate_run(ctx, rc, dg.get_lnv());
   mvgpu_get_timings(ctx, &rc.timings);
   mv_read_converged(ctx, rc);
   mv_print_scan_times(ctx, me);
@@ -128,10 +151,7 @@ inline GraphWeight distLouvainMethod(const int me, const int nprocs, const Graph
     rc.iter_trace.resize(n);
     if (n) mvgpu_get_trace(ctx, n, rc.iter_trace.data(), &n);
   }
-  if (rc.comm_out) {
-    rc.comm_out->resize(dg.get_lnv());
-    if (mvgpu_get_communities(ctx, rc.comm_out->data())) mv_abort("mvgpu_get_communities");
-  }
+  mv_result(ctx, rc, dg.get_lnv());
   mvgpu_destroy(ctx);
   return mod;
 }
@@ -159,7 +179,7 @@ inline GraphWeight distLouvainMethodOnDeviceRGG(const int me, const int nprocs, 
   double mod = 0.0;
   for (int rep = mv_env_repeat(); rep > 0; rep--)
     if (mvgpu_louvain(ctx, lower, thresh, &iters, &mod)) mv_abort("mvgpu_louvain");
-  mv_evaluate_run(ctx, rc);
+  mv_evaluate_run(ctx, rc, nv / nprocs);
   mvgpu_get_timings(ctx, &rc.timings);
   mv_read_converged(ctx, rc);
   mv_print_scan_times(ctx, me);
@@ -169,10 +189,7 @@ inline GraphWeight distLouvainMethodOnDeviceRGG(const int me, const int nprocs, 
     rc.iter_trace.resize(n);
     if (n) mvgpu_get_trace(ctx, n, rc.iter_trace.data(), &n);
   }
-  if (rc.comm_out) {
-    rc.comm_out->resize(nv / nprocs);
-    if (mvgpu_get_communities(ctx, rc.comm_out->data())) mv_abort("mvgpu_get_communities");
-  }
+  mv_result(ctx, rc, nv / nprocs);
   mvgpu_destroy(ctx);
   return mod;
 }

@@ -12,6 +12,8 @@
 //            iterations (prints STOPPED iters=<n> prevMod=<v>)   -L <v> starting `lower` (default -1; resume: -L <v>)
 //            -q evaluate the returned assignment (prints QUALITY mod=.. e=.. a2=.. communities=.. singletons=.. maxsize=..)
 //            -E <prefix> evaluate the communities an earlier -o <prefix> wrote, without a Louvain phase (prints QUALITY)
+//            -C split every community of the returned (or -E) assignment into its connected pieces; -q evaluates and -o
+//            writes the split assignment (prints SPLIT communities=.. components=.. disconnected=.. rounds=..)
 #include <getopt.h>
 #include <sys/mman.h>
 #include <sys/wait.h>
@@ -38,7 +40,7 @@ static int me = 0, nprocs = 1;
 static int ranksPerNode = 1;
 static GraphElem nvRGG = 0;
 static bool generateGraph = false, readBalanced = false, showGraph = false, traceIters = false, deviceGenerate = false,
-            evalQuality = false;
+            evalQuality = false, splitComm = false;
 static GraphWeight randomEdgePercent = 0.0;
 static bool randomNumberLCG = false, isUnitEdgeWeight = true;
 static GraphWeight threshold = 1.0E-6;
@@ -87,7 +89,7 @@ static long long reduce_sum_ll(long long v) {
 
 static void parseCommandLine(const int argc, char *const argv[]) {
   int ret;
-  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:")) != -1) {
+  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:C")) != -1) {
     switch (ret) {
       case 'f': inputFileName.assign(optarg); break;
       case 'b': readBalanced = true; break;
@@ -107,6 +109,7 @@ static void parseCommandLine(const int argc, char *const argv[]) {
       case 'L': lowerStart = atof(optarg); break;
       case 'q': evalQuality = true; break;
       case 'E': evalPrefix.assign(optarg); break;
+      case 'C': splitComm = true; break;
       default: assert(0 && "Option not recognized!!!"); break;
     }
   }
@@ -265,6 +268,7 @@ int main(int argc, char *argv[]) {
   }
   rc.stop_after = stopAfter;
   rc.quality = evalQuality;
+  rc.split = splitComm;
 
   GraphWeight currMod = lowerStart;
   std::vector<GraphElem> ssizes, rsizes, svdata, rvdata;
@@ -296,6 +300,9 @@ int main(int argc, char *argv[]) {
   const double total = wtime() - t1;
   const double tot_time = reduce_sum(total);
   const double dev_time = reduce_sum(rc.timings.total_s);
+  if (me == 0 && splitComm)
+    fprintf(stderr, "SPLIT communities=%ld components=%ld disconnected=%ld rounds=%d\n", (long)rc.split_rep.communities,
+            (long)rc.split_rep.components, (long)rc.split_rep.disconnected, (int)rc.split_rep.rounds);
   if (me == 0 && (evalQuality || !evalPrefix.empty()))
     fprintf(stderr, "QUALITY mod=%.17g e=%.17g a2=%.17g communities=%ld singletons=%ld maxsize=%ld\n", rc.q.modularity,
             rc.q.e_in, rc.q.a2, (long)rc.q.communities, (long)rc.q.singletons, (long)rc.q.max_size);

@@ -1419,4 +1419,113 @@ __global__ void __launch_bounds__(256) k_q_labels(int lnv, const int32_t *X, Pee
   }
 }
 
+// ----------------------------------------------------------------------------------------------
+// Connected components inside the communities of an assignment (mvgpu_split_communities, DESIGN.md §3.12).  setup_run
+// has left cur = X on every slot, without renumbering (internal ids are caller ids).  lab[v] is a global vertex id that
+// only decreases and always names a vertex of v's component; hooking and pointer jumping repeat until no label changes
+// on any rank, and then every vertex holds the smallest id of its component.  Labels are read with ld.global.cg: peers
+// lower them concurrently, and a round that reads a stale value only does less work.
+// ----------------------------------------------------------------------------------------------
+struct SplitPeers {                                 // every rank's labels (peer mappings for other ranks)
+  int32_t *lab[kMaxRanks];
+};
+
+// the label entry of global vertex id y: this rank's array lab for an owned id, the owner's (peer memory) otherwise
+__device__ __forceinline__ int32_t *split_lab_at(const PeerTable &pt, const SplitPeers &sp, int32_t *lab, long long base, int lnv,
+                                                 int y) {
+  const long long i = (long long)y - base;
+  if ((unsigned long long)i < (unsigned long long)lnv) return lab + i;
+  int o; long long idx;
+  locate_remote(pt, y, o, idx);
+  return sp.lab[o] + idx;
+}
+
+__global__ void __launch_bounds__(256) k_split_init(int lnv, long long base, int32_t *lab) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) lab[v] = (int32_t)(base + v);
+}
+
+// the row of record e: the last v in [lo, hi] with rowptr[v] <= e
+__device__ __forceinline__ int split_row_of(const uint32_t *rowptr, int lo, int hi, long long e) {
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if ((long long)rowptr[mid] <= e) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// Hook, one thread per record i -> t with X(i) = X(t) and t != i: the larger of the two labels is a vertex id, and its
+// label entry (at its owner) takes the smaller one by atomicMin.  Blocks walk 256-record tiles; the tile's first and
+// last rows bound every thread's row search, so a tile inside one long adjacency list (a hub) searches nothing.
+// acc->moved counts the labels this launch lowered.
+__global__ void __launch_bounds__(256) k_split_hook(int lnv, long long base, const uint32_t *rowptr, const int32_t *tails,
+                                                    const int32_t *cur, const long long *ghost_gid, int32_t *lab, PeerTable pt,
+                                                    SplitPeers sp, Acc *acc) {
+  __shared__ int rows[2];
+  const long long lne = rowptr[lnv];
+  unsigned long long lowered = 0;
+  for (long long t0 = (long long)blockIdx.x * 256; t0 < lne; t0 += (long long)gridDim.x * 256) {
+    if (threadIdx.x < 2) rows[threadIdx.x] = split_row_of(rowptr, 0, lnv - 1, threadIdx.x ? min(t0 + 255, lne - 1) : t0);
+    __syncthreads();
+    const long long e = t0 + threadIdx.x;
+    if (e < lne) {
+      const int i = split_row_of(rowptr, rows[0], rows[1], e);
+      const int t = tails[e];
+      if (t != i && cur[t] == cur[i]) {
+        const int li = __ldcg(lab + i);
+        const int lt = __ldcg(t < lnv ? lab + t : split_lab_at(pt, sp, lab, base, lnv, (int)ghost_gid[t - lnv]));
+        if (li != lt) {
+          const int lo = min(li, lt);
+          if (atomicMin(split_lab_at(pt, sp, lab, base, lnv, max(li, lt)), lo) > lo) lowered++;
+        }
+      }
+    }
+    __syncthreads();
+  }
+  lowered = warp_sum(lowered);
+  if ((threadIdx.x & 31) == 0 && lowered) atomicAdd(&acc->moved, lowered);
+}
+
+// Shortcut: lab[v] = lab[lab[v]] (one pointer jump, the second read at the label's owner); counts into acc->moved
+__global__ void __launch_bounds__(256) k_split_jump(int lnv, long long base, int32_t *lab, PeerTable pt, SplitPeers sp, Acc *acc) {
+  unsigned long long lowered = 0;
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) {
+    const int l = __ldcg(lab + v);
+    if ((long long)l == base + v) continue;
+    const int ll = __ldcg(split_lab_at(pt, sp, lab, base, lnv, l));
+    if (ll < l && atomicMin(lab + v, ll) > ll) lowered++;
+  }
+  lowered = warp_sum(lowered);
+  if ((threadIdx.x & 31) == 0 && lowered) atomicAdd(&acc->moved, lowered);
+}
+
+// every component root (lab[v] = v) adds 1 to the counter of its community X(v) at the community's owner (the
+// evaluation's q.internal array, as uint64, zeroed by init_state)
+__global__ void __launch_bounds__(256) k_split_roots(int lnv, long long base, const int32_t *cur, const int32_t *lab, PeerTable pt,
+                                                     QualPeers q) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < lnv; v += gridDim.x * blockDim.x) {
+    if ((long long)__ldcg(lab + v) != base + v) continue;
+    int o; long long idx;
+    locate_remote(pt, cur[v], o, idx);
+    atomicAdd(reinterpret_cast<unsigned long long *>(q.internal[o]) + idx, 1ULL);
+  }
+}
+
+// over the owned communities: agg[0] += non-empty ones (counter >= 1), agg[1] += components, agg[2] += disconnected
+// ones (counter >= 2)
+__global__ void __launch_bounds__(256) k_split_count(int lnv, const unsigned long long *cnt, unsigned long long *agg) {
+  unsigned long long nonempty = 0, comps = 0, split = 0;
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < lnv; s += gridDim.x * blockDim.x) {
+    const unsigned long long k = cnt[s];
+    nonempty += k != 0;
+    comps += k;
+    split += k > 1;
+  }
+  nonempty = warp_sum(nonempty); comps = warp_sum(comps); split = warp_sum(split);
+  if ((threadIdx.x & 31) == 0) {
+    if (nonempty) atomicAdd(&agg[0], nonempty);
+    if (comps) atomicAdd(&agg[1], comps);
+    if (split) atomicAdd(&agg[2], split);
+  }
+}
+
 }  // namespace mv

@@ -104,7 +104,8 @@ struct DevBuf {              // grow-only device buffer (allocations are cached 
   X(p2p, true, 1, c->pp.st[r])                                      \
   X(inv, c->relabel, need_v, c->peer_inv[r])                        \
   X(q_internal, true, ev ? need_v : 0, c->qp.internal[r])           \
-  X(q_rank, true, ev ? need_v + 1 : 0, c->qp.rank[r])
+  X(q_rank, true, ev ? need_v + 1 : 0, c->qp.rank[r])                \
+  X(split_lab, true, split ? need_v : 0, c->spp.lab[r])
 #define MV_COUNT(...) +1
 constexpr int kPeerArrays = 0 MV_EXPORTS(MV_COUNT);
 #undef MV_COUNT
@@ -234,6 +235,9 @@ struct mvgpu_ctx {
   DevBuf<int32_t> q_rank, q_flag, q_lab;
   DevBuf<long long> q_size;
   QualPeers qp;
+  // splitting (mvgpu_split_communities): labels, peer-exported; the counters reuse q_internal
+  DevBuf<int32_t> split_lab;
+  SplitPeers spp;
   bool run_on_shard = false;           // final_orig holds a run's assignment of the current shard
   bool eval_on_shard = false;          // the q_* arrays describe an evaluation of the current shard
   // results
@@ -286,6 +290,7 @@ struct Scalars {
   long long counts[2 * kMaxRanks];
   unsigned long long span_sum, span_cnt;
   unsigned long long q_agg[2];         // evaluation: singletons, largest community
+  unsigned long long split_agg[3];     // splitting: non-empty communities, components, disconnected communities
 };
 Scalars *dev_scalars(mvgpu_ctx *c) { return reinterpret_cast<Scalars *>(c->scratch.p); }
 
@@ -397,7 +402,8 @@ int cub_run(mvgpu_ctx *c, F &&...f) {
 
 // ---- multi-GPU: publish/obtain peer pointers for the exported arrays (MV_EXPORTS) ------------------------------------
 // this rank's exported arrays, in MV_EXPORTS order (the sizes matter to the grow test of setup_agree only)
-void exports(const mvgpu_ctx *c, Export (&x)[kPeerArrays], size_t need_v = 0, size_t need_s = 0, bool ev = false) {
+void exports(const mvgpu_ctx *c, Export (&x)[kPeerArrays], size_t need_v = 0, size_t need_s = 0, bool ev = false,
+             bool split = false) {
   int k = 0;
 #define MV_EXPORT(buf, on, need, dst) x[k++] = {(on) ? (void *)c->buf.p : nullptr, c->buf.gen, c->buf.cap, (size_t)(need)};
   MV_EXPORTS(MV_EXPORT)
@@ -592,6 +598,7 @@ int warm_init(mvgpu_ctx *c, const int32_t *init) {
 struct EvalSetup {
   const int32_t *X = nullptr;
   bool given = false;                  // the caller passed an array (not NULL)
+  bool split = false;                  // for mvgpu_split_communities: the labels are allocated and exported too
   std::string err;
 };
 
@@ -639,7 +646,7 @@ int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, 
     // CUDA IPC requires every peer to close its mapping before the owner frees the block, so growing an exported array
     // is agreed on here and done collectively (need_s: init_state's bound lnv + #non-owned edge tails >= lnv + nghost)
     Export x[kPeerArrays];
-    exports(c, x, (size_t)c->lnv, (size_t)(c->lnv + nremote), ev != nullptr);
+    exports(c, x, (size_t)c->lnv, (size_t)(c->lnv + nremote), ev != nullptr, ev && ev->split);
     bool grow = false;
     for (const Export &e : x) grow = grow || (c->ipc_valid && e.cap && e.cap < e.need);
     const bool assigned = ev ? ev->given : c->warm_run;
@@ -649,7 +656,8 @@ int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, 
     ne_global = hv[1];
     if (hv[2] && err.empty()) err = ev ? "another rank rejected its shard or its assignment" : "another rank rejected its shard";
     if (err.empty() && hv[4] != 0 && hv[4] != c->nranks)
-      err = ev ? "ranks disagree on the assignment to evaluate: every rank or none must pass NULL"
+      err = ev ? (ev->split ? "ranks disagree on the assignment to split: every rank or none must pass NULL"
+                            : "ranks disagree on the assignment to evaluate: every rank or none must pass NULL")
                : "ranks disagree on the initial assignment: every rank or none must set one";
     if (hv[3]) {
       close_ipc(c);
@@ -876,6 +884,7 @@ int init_state(mvgpu_ctx *c, const EvalSetup *ev, long long nremote) {
   if (ev) {                                   // zeroed before warm_init's last barrier: no peer adds to it earlier
     TRY(c->q_internal.ensure(lnv)); TRY(c->q_rank.ensure(lnv + 1));
     CK(cudaMemsetAsync(c->q_internal.p, 0, sizeof(double) * lnv, s));
+    if (ev->split) TRY(c->split_lab.ensure(lnv));
   }
   if (c->unit)
     k_vertex_init<true><<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->base, c->a_rowptr, c->a_tails, nullptr, c->comm_a.p,
@@ -1301,50 +1310,147 @@ std::string narrow_ids(const mvgpu_ctx *c, const int64_t *comm, const char *who,
   return "";
 }
 
-// collective: every rank calls it with an array or every rank with NULL.  caller_err: a finding of the caller's own
-// (a binding that could not build the array), which fails the call on every rank like a bad id
-int evaluate(mvgpu_ctx *c, const int64_t *comm, mvgpu_quality *out, const char *caller_err = nullptr) {
-  TRY(check_ready(c));
-  CK(cudaSetDevice(c->device));
-  cudaStream_t s = c->stream;
-  c->eval_on_shard = false;                    // the q_* arrays are rewritten from here on
-  // The last run's assignment in caller order is resolved while comm_a / comm_b still hold it (one-rank runs leave it
-  // unresolved; setup_run below overwrites comm_a), whatever is evaluated: communities(), get_communities_device and a
-  // later NULL evaluation read final_orig, which an evaluation never writes.
-  if (c->run_on_shard) TRY(final_in_caller_order(c));
-  EvalSetup ev;
+// The assignment an evaluation or a split reads: comm (validated and copied to eval_comm) or, for NULL, the last run's
+// result in caller order (resolved by the caller of this).  Local findings are not returned here: they go into ev.err,
+// prefixed by `who`, and join setup_run's input agreement, so that every rank fails together.  caller_err: a finding of
+// the caller's own (a binding that could not build the array), which fails the call on every rank like a bad id.
+int take_assignment(mvgpu_ctx *c, const int64_t *comm, const char *who, const char *verb, const char *caller_err, EvalSetup &ev) {
+  const std::string w(who);
   ev.given = comm != nullptr;
-  // local findings are not returned here: they join setup_run's input agreement, so that every rank fails together
-  if (caller_err) ev.err = std::string("mvgpu_evaluate_communities: ") + caller_err;
-  else if (c->f32) ev.err = "mvgpu_evaluate_communities: not for a shard uploaded with mvgpu_upload_shard32";
-  else if (!comm && !c->run_on_shard) ev.err = "mvgpu_evaluate_communities: NULL evaluates the last mvgpu_louvain result, and there is none on this shard";
+  if (caller_err) ev.err = w + ": " + caller_err;
+  else if (c->f32) ev.err = w + ": not for a shard uploaded with mvgpu_upload_shard32";
+  else if (!comm && !c->run_on_shard) ev.err = w + ": NULL " + verb + " the last mvgpu_louvain result, and there is none on this shard";
   else if (comm) {
     std::vector<int32_t> h;
-    ev.err = narrow_ids(c, comm, "mvgpu_evaluate_communities", h);
+    ev.err = narrow_ids(c, comm, who, h);
     if (ev.err.empty()) {
       TRY(c->eval_comm.ensure(c->lnv));
-      if (c->lnv) CK(cudaMemcpyAsync(c->eval_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice, s));
-      CK(cudaStreamSynchronize(s));
+      if (c->lnv) CK(cudaMemcpyAsync(c->eval_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice, c->stream));
+      CK(cudaStreamSynchronize(c->stream));
       ev.X = c->eval_comm.p;
     }
   } else {
     ev.X = c->final_orig.p;
   }
+  return 0;
+}
+
+// setup_run(ev), then pass(), between two events on the stream (seconds: the device time between them); leaves
+// everything the last run reports as it was
+template <typename F>
+int assignment_pass(mvgpu_ctx *c, const EvalSetup &ev, F &&pass, double &seconds) {
+  cudaStream_t s = c->stream;
   const RunReport saved = save_report(c);
   memset(&c->tm, 0, sizeof c->tm);
   c->peers_ready = false;                      // the evaluation's tables differ from the run's (no labels, q arrays)
   cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
   int rc = cudaEventRecord(e0, s) == cudaSuccess ? 0 : fail("cudaEventRecord");
   if (!rc) rc = setup_run(c, &ev);
-  if (!rc) rc = evaluate_pass(c, ev.X, out);
+  if (!rc) rc = pass();
   if (!rc && cudaEventRecord(e1, s) != cudaSuccess) rc = fail("cudaEventRecord");
   if (!rc && cudaEventSynchronize(e1) != cudaSuccess) rc = fail("cudaEventSynchronize");
   float ms = 0;
   if (!rc && cudaEventElapsedTime(&ms, e0, e1) != cudaSuccess) rc = fail("cudaEventElapsedTime");
-  if (!rc) out->eval_s = ms * 1e-3;
+  if (!rc) seconds = ms * 1e-3;
   restore_report(c, saved);
   c->peers_ready = false;                      // the next run rebuilds its own tables
   return rc;
+}
+
+// collective: every rank calls it with an array or every rank with NULL
+int evaluate(mvgpu_ctx *c, const int64_t *comm, mvgpu_quality *out, const char *caller_err = nullptr) {
+  TRY(check_ready(c));
+  CK(cudaSetDevice(c->device));
+  c->eval_on_shard = false;                    // the q_* arrays are rewritten from here on
+  // The last run's assignment in caller order is resolved while comm_a / comm_b still hold it (one-rank runs leave it
+  // unresolved; setup_run below overwrites comm_a), whatever is evaluated: communities(), get_communities_device and a
+  // later NULL evaluation read final_orig, which an evaluation never writes.
+  if (c->run_on_shard) TRY(final_in_caller_order(c));
+  EvalSetup ev;
+  TRY(take_assignment(c, comm, "mvgpu_evaluate_communities", "evaluates", caller_err, ev));
+  return assignment_pass(c, ev, [&] { return evaluate_pass(c, ev.X, out); }, out->eval_s);
+}
+
+// ---- splitting (DESIGN.md §3.12): after setup_run(ev), comm_a = X on every slot; the labels end in split_lab ----------
+// Labels only decrease, so the loop ends; the cap turns a defect into an error instead of a hang.
+constexpr int kSplitMaxRounds = 1000;
+
+int split_pass(mvgpu_ctx *c, mvgpu_split_report *rep) {
+  cudaStream_t s = c->stream;
+  const int lnv = (int)c->lnv, nsm = c->num_sms;
+  Scalars *d_sc = dev_scalars(c);
+  Acc *acc = c->acc.p + 1;                     // one record, cleared every round (record 0 holds the warm fold's a2)
+  if (lnv > 0) {
+    k_split_init<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->base, c->split_lab.p);
+    c->tm.kernel_launches++;
+  }
+  TRY(run_barrier(c));                         // every rank's labels are set before a peer reads or lowers them
+  int rounds = 0;
+  for (;;) {
+    if (rounds == kSplitMaxRounds)
+      return fail("mvgpu_split_communities: labels still changing after " + std::to_string(kSplitMaxRounds) + " rounds");
+    rounds++;
+    CK(cudaMemsetAsync(acc, 0, sizeof(Acc), s));
+    if (c->lne > 0) {
+      k_split_hook<<<grid_for(c->lne, 256, nsm), 256, 0, s>>>(lnv, c->base, c->a_rowptr, c->a_tails, c->comm_a.p, c->ghost_gid.p,
+                                                              c->split_lab.p, c->pt, c->spp, acc);
+      c->tm.kernel_launches++;
+    }
+    TRY(run_barrier(c));                       // the round's hooks have landed on every rank before labels jump
+    if (lnv > 0) {
+      k_split_jump<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->base, c->split_lab.p, c->pt, c->spp, acc);
+      c->tm.kernel_launches++;
+    }
+    TRY(acc_sum_enqueue(c, acc, true));        // labels lowered this round, summed over the ranks (acc->moved)
+    CK(cudaStreamSynchronize(s));
+    AccSum sum;
+    TRY(acc_sum_read(c, sum));
+    if (sum.moved == 0) break;                 // the same on every rank: every rank leaves the loop after this round
+  }
+  if (lnv > 0) {
+    k_split_roots<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->base, c->comm_a.p, c->split_lab.p, c->pt, c->qp);
+    c->tm.kernel_launches++;
+  }
+  // every root has been counted at its community's owner; from here on no rank touches a peer's arrays, so each may
+  // leave the call when it is done
+  TRY(run_barrier(c));
+  CK(cudaMemsetAsync(d_sc->split_agg, 0, sizeof d_sc->split_agg, s));
+  if (lnv > 0) {
+    k_split_count<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, reinterpret_cast<const unsigned long long *>(c->q_internal.p),
+                                                          d_sc->split_agg);
+    c->tm.kernel_launches++;
+  }
+  unsigned long long agg[3];
+  CK(cudaMemcpyAsync(agg, d_sc->split_agg, sizeof agg, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  long long tot[3] = {(long long)agg[0], (long long)agg[1], (long long)agg[2]};
+  TRY(coll_allreduce_i64(c, tot, 3, false));
+  rep->communities = tot[0]; rep->components = tot[1]; rep->disconnected = tot[2]; rep->rounds = rounds;
+  return 0;
+}
+
+// collective like evaluate; out is written only when the call succeeds
+int split(mvgpu_ctx *c, const int64_t *comm, int64_t *out, mvgpu_split_report *rep, const char *caller_err = nullptr) {
+  TRY(check_ready(c));
+  CK(cudaSetDevice(c->device));
+  c->eval_on_shard = false;                    // the split counts components in the evaluation's q_internal
+  if (c->run_on_shard) TRY(final_in_caller_order(c));   // as in evaluate: setup_run overwrites comm_a
+  EvalSetup ev;
+  ev.split = true;
+  TRY(take_assignment(c, comm, "mvgpu_split_communities", "splits", caller_err, ev));
+  mvgpu_split_report r;
+  memset(&r, 0, sizeof r);
+  TRY(assignment_pass(c, ev, [&] { return split_pass(c, &r); }, r.split_s));
+  if (c->lnv > 0) {
+    TRY(c->wide.ensure(c->lnv));
+    k_widen<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(c->split_lab.p, c->lnv, c->wide.p);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * c->lnv, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+  }
+  *rep = r;
+  return 0;
 }
 
 // ---- shard update (DESIGN.md §3.11, merge_gpu.cuh) -------------------------------------------------------------------
@@ -1926,6 +2032,18 @@ int mvgpu_evaluate_communities(mvgpu_ctx *c, const int64_t *comm, mvgpu_quality 
 int mv_evaluate_refused(mvgpu_ctx *c, const char *why, mvgpu_quality *out) {
   if (!c || !out || !why) return fail("null argument");
   return evaluate(c, nullptr, out, why);
+}
+
+int mvgpu_split_communities(mvgpu_ctx *c, const int64_t *comm, int64_t *out, mvgpu_split_report *rep) {
+  if (!c || !out || !rep) return fail("null argument");
+  return split(c, comm, out, rep);
+}
+
+// Not in mvgpu.h: the Python binding's way into the collective when it cannot build the array, as mv_evaluate_refused
+int mv_split_refused(mvgpu_ctx *c, const char *why, mvgpu_split_report *rep) {
+  if (!c || !rep || !why) return fail("null argument");
+  int64_t none = 0;
+  return split(c, nullptr, &none, rep, why);
 }
 
 int mvgpu_get_community_stats(mvgpu_ctx *c, int64_t *size, double *volume, double *internal) {

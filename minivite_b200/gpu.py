@@ -35,13 +35,21 @@ class Quality(ctypes.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class SplitReport(ctypes.Structure):
+    _fields_ = [("communities", ctypes.c_int64), ("components", ctypes.c_int64), ("disconnected", ctypes.c_int64),
+                ("rounds", ctypes.c_int32), ("split_s", ctypes.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_destroy", "mvgpu_get_unique_id",
            "mvgpu_comm_init", "mvgpu_upload_shard", "mvgpu_attach_shard_device", "mvgpu_generate_rgg_shard", "mvgpu_generate_rgg_shard_ex",
            "mvgpu_download_shard", "mvgpu_louvain",
            "mvgpu_get_communities", "mvgpu_get_communities_device", "mvgpu_upload_shard32", "mvgpu_louvain32", "mvgpu_get_communities32", "mvgpu_set_option", "mvgpu_get_trace",
            "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method",
            "mvgpu_set_initial_communities", "mvgpu_get_converged", "mvgpu_evaluate_communities",
-           "mvgpu_get_community_stats", "mvgpu_get_compact_communities", "mvgpu_update_shard"]
+           "mvgpu_get_community_stats", "mvgpu_get_compact_communities", "mvgpu_update_shard", "mvgpu_split_communities"]
 
 _lib = None
 
@@ -73,6 +81,8 @@ def lib():
         L.mvgpu_evaluate_communities.argtypes = [vp, vp, ctypes.POINTER(Quality)]
         L.mv_evaluate_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(Quality)]
         L.mvgpu_get_community_stats.argtypes = [vp, vp, vp, vp]
+        L.mvgpu_split_communities.argtypes = [vp, vp, vp, ctypes.POINTER(SplitReport)]
+        L.mv_split_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(SplitReport)]
         L.mvgpu_get_compact_communities.argtypes = [vp, vp]
         L.mvgpu_upload_shard32.argtypes = [vp, ctypes.c_int32, vp, ctypes.c_int32, ctypes.c_int32, vp, vp]
         L.mvgpu_louvain32.argtypes = [vp, ctypes.c_float, ctypes.c_float, ctypes.POINTER(ci), ctypes.POINTER(ctypes.c_float)]
@@ -259,6 +269,27 @@ class LouvainGPU:
         buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
         _ck(lib().mvgpu_evaluate_communities(self._h, buf.ctypes.data, ctypes.byref(q)))
         return q.as_dict()
+
+    def split_communities(self, comm=None):
+        """Split every community of an assignment into its connected pieces (DESIGN.md §3.12): Y gives each vertex the
+        smallest global id of its component, where two vertices are joined when they share a community and the shard
+        stores a record between them.  `comm` takes the form evaluate() takes; None splits what the last louvain()
+        returned.  Collective, with evaluate()'s error rules.  Returns (Y, report): Y is this rank's lnv entries (int64,
+        a valid input to set_initial_communities and evaluate), report the global counts of mvgpu_split_report as a dict."""
+        rep = SplitReport()
+        out = np.zeros(max(self.lnv, 1), np.int64)
+        if comm is None:
+            _ck(lib().mvgpu_split_communities(self._h, None, out.ctypes.data, ctypes.byref(rep)))
+            return out[:self.lnv], rep.as_dict()
+        comm = np.ascontiguousarray(comm, dtype=np.int64)
+        if comm.ndim != 1 or comm.size != self.lnv:
+            # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
+            why = f"assignment has {comm.size} entries, the shard has lnv = {self.lnv}"
+            _ck(lib().mv_split_refused(self._h, why.encode(), ctypes.byref(rep)))
+            raise AssertionError("unreachable: a refused split fails")
+        buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
+        _ck(lib().mvgpu_split_communities(self._h, buf.ctypes.data, out.ctypes.data, ctypes.byref(rep)))
+        return out[:self.lnv], rep.as_dict()
 
     def community_stats(self):
         """Per community of the last evaluate(): entry s describes community parts[rank] + s.  Returns a dict of
