@@ -177,6 +177,36 @@ typedef struct {
  * were; the per-community arrays of the last evaluation are gone (their getters fail until the next evaluation). */
 int mvgpu_split_communities(mvgpu_ctx *ctx, const int64_t *comm, int64_t *out, mvgpu_split_report *rep);
 
+/* ---- comparing two assignments (DESIGN.md §3.13) ---------------------------------------------------------------------
+ * X and Y give every vertex a community id in [0, nv).  n_xy = #{v : X(v) = x, Y(v) = y} (a cell), a_x = |x|, b_y = |y|.
+ * The counts are exact: pairs_xy = sum C(n_xy, 2), pairs_x = sum C(a_x, 2), pairs_y = sum C(b_y, 2), pairs_all = C(N, 2)
+ * with N = nv; cells = the non-zero n_xy.  The doubles follow from them on the host in a fixed order, so every field is
+ * the same bit for bit on every rank count:
+ *   ari  = den == 0 ? 1 : num / den, num = 2 (pairs_all pairs_xy - pairs_x pairs_y),
+ *          den = pairs_all (pairs_x + pairs_y) - 2 pairs_x pairs_y (exact 128-bit integers, one rounding each)
+ *   rand = (pairs_all + 2 pairs_xy - pairs_x - pairs_y) / pairs_all (1 when pairs_all = 0)
+ *   S(h) = sum over the values k > 1 of a histogram, ascending, of m_k (k log k); h_x = log N - S(a) / N (0 for at most
+ *          one community), h_y likewise, mi = log N + (S(n) - (S(a) + S(b))) / N (0 when X or Y has at most one
+ *          community), nmi = 2 mi / (h_x + h_y) (1 when h_x + h_y = 0; the arithmetic normalisation), vi = h_x + h_y - 2 mi */
+typedef struct {
+  int64_t vertices, communities_x, communities_y, cells;
+  uint64_t pairs_xy, pairs_x, pairs_y, pairs_all;
+  double ari, rand, nmi, vi, mi, h_x, h_y;
+  double compare_s; /* device time of the call once both arrays are on the device (CUDA events on the context's stream) */
+} mvgpu_compare_report;
+/* Collective.  x, y: lnv community ids each in the caller's vertex numbering (the form mvgpu_evaluate_communities
+ * takes); x = NULL compares the assignment the last mvgpu_louvain on this shard returned; y must not be NULL.  A bad id
+ * in either array, NULL x without a run, ranks that disagree on NULL or a shard from mvgpu_upload_shard32 fail the call
+ * on every rank, and then nothing is written.  Reads none of the shard's edges, and leaves everything the last run
+ * reports, the initial assignment and the last evaluation's per-community arrays as they were. */
+int mvgpu_compare_communities(mvgpu_ctx *ctx, const int64_t *x, const int64_t *y, mvgpu_compare_report *rep);
+/* Per community x of the last successful compare: entry s describes community parts[rank] + s (the layout of
+ * mvgpu_get_community_stats).  size = a_x; best = the y with the largest n_xy, ties to the smallest y; overlap = n_x,best;
+ * best_size = b_best (Jaccard = overlap / (size + best_size - overlap)).  An empty x has size 0, best -1, overlap 0,
+ * best_size 0.  The reverse direction is the compare with x and y swapped.  Fails before the first compare, after a
+ * failed one, and after the next upload, attach or generate.  Any of the four arrays may be NULL (not written). */
+int mvgpu_get_community_matches(mvgpu_ctx *ctx, int64_t *size, int64_t *best, int64_t *overlap, int64_t *best_size);
+
 /* currComm of this rank's vertices at exit (global community ids), lnv entries. */
 int mvgpu_get_communities(mvgpu_ctx *ctx, int64_t *out);
 /* Same values left in device memory (int32 global ids); valid until the next mvgpu_louvain. */

@@ -31,6 +31,8 @@ struct GpuRankContext {
   bool split = false;                                  // -C: split the run's (or -E's) assignment into connected pieces
   mvgpu_split_report split_rep{};                      // -C: the split's counts (global values)
   std::vector<GraphElem> split_comm;                   // -C: the split assignment of this rank's vertices
+  const std::vector<GraphElem> *cmp_comm = nullptr;    // -M: compare the assignment -q would evaluate with this one
+  mvgpu_compare_report cmp{};                          // -M: the comparison (global values)
 };
 
 [[noreturn]] inline void mv_abort(const std::string &where) {
@@ -75,6 +77,13 @@ inline void mv_split(mvgpu_ctx *ctx, GpuRankContext &rc, const GraphElem *comm, 
   if (mvgpu_split_communities(ctx, comm, rc.split_comm.data(), &rc.split_rep)) mv_abort("mvgpu_split_communities");
   rc.split_comm.resize(lnv);
 }
+// -M: compare X (NULL: the run's result) with the assignment read from -M's files
+inline void mv_compare(mvgpu_ctx *ctx, GpuRankContext &rc, const GraphElem *X) {
+  if (!rc.cmp_comm) return;
+  const GraphElem none = 0;                        // an empty shard still passes a non-NULL array
+  const GraphElem *Y = rc.cmp_comm->empty() ? &none : rc.cmp_comm->data();
+  if (mvgpu_compare_communities(ctx, X, Y, &rc.cmp)) mv_abort("mvgpu_compare_communities");
+}
 // -E: evaluate the given assignment (with -C: its split) and run no Louvain phase (true: done, the caller returns)
 inline bool mv_evaluate_only(mvgpu_ctx *ctx, GpuRankContext &rc) {
   if (!rc.eval_comm) return false;
@@ -83,13 +92,15 @@ inline bool mv_evaluate_only(mvgpu_ctx *ctx, GpuRankContext &rc) {
     mv_split(ctx, rc, X, (GraphElem)rc.eval_comm->size());
     X = rc.split_comm.data();
   }
+  mv_compare(ctx, rc, X);
   if (mvgpu_evaluate_communities(ctx, X, &rc.q)) mv_abort("mvgpu_evaluate_communities");
   mvgpu_destroy(ctx);
   return true;
 }
-// -C: split the assignment the run returned; -q: evaluate the run's assignment (with -C: its split)
+// -C: split the assignment the run returned; -M: compare the run's assignment (with -C: its split); -q: evaluate it
 inline void mv_evaluate_run(mvgpu_ctx *ctx, GpuRankContext &rc, GraphElem lnv) {
   if (rc.split) mv_split(ctx, rc, nullptr, lnv);
+  mv_compare(ctx, rc, rc.split ? rc.split_comm.data() : nullptr);
   if (rc.quality && mvgpu_evaluate_communities(ctx, rc.split ? rc.split_comm.data() : nullptr, &rc.q))
     mv_abort("mvgpu_evaluate_communities");
 }

@@ -14,6 +14,8 @@
 //            -E <prefix> evaluate the communities an earlier -o <prefix> wrote, without a Louvain phase (prints QUALITY)
 //            -C split every community of the returned (or -E) assignment into its connected pieces; -q evaluates and -o
 //            writes the split assignment (prints SPLIT communities=.. components=.. disconnected=.. rounds=..)
+//            -M <prefix> compare the assignment -q would evaluate with the communities an earlier -o <prefix> wrote
+//            (prints COMPARE ari=.. nmi=.. vi=.. rand=.. mi=.. hx=.. hy=.. cells=.. communities_x=.. communities_y=..)
 #include <getopt.h>
 #include <sys/mman.h>
 #include <sys/wait.h>
@@ -33,7 +35,7 @@
 #include "louvain.hpp"
 #include "rgg.hpp"
 
-static std::string inputFileName, dumpPrefix, initPrefix, evalPrefix;
+static std::string inputFileName, dumpPrefix, initPrefix, evalPrefix, comparePrefix;
 static int stopAfter = 0;
 static GraphWeight lowerStart = -1.0;
 static int me = 0, nprocs = 1;
@@ -89,7 +91,7 @@ static long long reduce_sum_ll(long long v) {
 
 static void parseCommandLine(const int argc, char *const argv[]) {
   int ret;
-  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:C")) != -1) {
+  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:CM:")) != -1) {
     switch (ret) {
       case 'f': inputFileName.assign(optarg); break;
       case 'b': readBalanced = true; break;
@@ -110,6 +112,7 @@ static void parseCommandLine(const int argc, char *const argv[]) {
       case 'q': evalQuality = true; break;
       case 'E': evalPrefix.assign(optarg); break;
       case 'C': splitComm = true; break;
+      case 'M': comparePrefix.assign(optarg); break;
       default: assert(0 && "Option not recognized!!!"); break;
     }
   }
@@ -257,7 +260,7 @@ int main(int argc, char *argv[]) {
               "shard {base %lld, lnv %lld}\n", flag, prefix.c_str(), fn.c_str(), hdr[0], hdr[1], want_base, want_lnv);
     if (reduce_sum_ll(ok ? 0 : 1)) abort_all(99);       // every rank leaves, not only the one with the bad file
   };
-  std::vector<GraphElem> initComm, evalComm;
+  std::vector<GraphElem> initComm, evalComm, cmpComm;
   if (!initPrefix.empty()) {
     read_assignment("-i", initPrefix, initComm);
     rc.init_comm = &initComm;
@@ -265,6 +268,10 @@ int main(int argc, char *argv[]) {
   if (!evalPrefix.empty()) {
     read_assignment("-E", evalPrefix, evalComm);
     rc.eval_comm = &evalComm;
+  }
+  if (!comparePrefix.empty()) {
+    read_assignment("-M", comparePrefix, cmpComm);
+    rc.cmp_comm = &cmpComm;
   }
   rc.stop_after = stopAfter;
   rc.quality = evalQuality;
@@ -303,6 +310,10 @@ int main(int argc, char *argv[]) {
   if (me == 0 && splitComm)
     fprintf(stderr, "SPLIT communities=%ld components=%ld disconnected=%ld rounds=%d\n", (long)rc.split_rep.communities,
             (long)rc.split_rep.components, (long)rc.split_rep.disconnected, (int)rc.split_rep.rounds);
+  if (me == 0 && !comparePrefix.empty())
+    fprintf(stderr, "COMPARE ari=%.17g nmi=%.17g vi=%.17g rand=%.17g mi=%.17g hx=%.17g hy=%.17g cells=%ld communities_x=%ld "
+            "communities_y=%ld\n", rc.cmp.ari, rc.cmp.nmi, rc.cmp.vi, rc.cmp.rand, rc.cmp.mi, rc.cmp.h_x, rc.cmp.h_y,
+            (long)rc.cmp.cells, (long)rc.cmp.communities_x, (long)rc.cmp.communities_y);
   if (me == 0 && (evalQuality || !evalPrefix.empty()))
     fprintf(stderr, "QUALITY mod=%.17g e=%.17g a2=%.17g communities=%ld singletons=%ld maxsize=%ld\n", rc.q.modularity,
             rc.q.e_in, rc.q.a2, (long)rc.q.communities, (long)rc.q.singletons, (long)rc.q.max_size);

@@ -21,6 +21,7 @@
 #include <cstdio>
 #include <cstring>
 #include <cub/cub.cuh>
+#include <map>
 #include <random>
 #include <string>
 #include <thread>
@@ -35,6 +36,7 @@
 #include "nccl_dyn.h"
 #include "rgg_gpu.cuh"
 #include "merge_gpu.cuh"
+#include "compare_gpu.cuh"
 
 // host-only helper of the compact upload (narrow.cpp): 16-byte edge records -> 4-byte tails + validation
 extern "C" void mv_narrow_edges(const void *edge_records, long long n, long long nv, long long base, long long bound,
@@ -238,8 +240,17 @@ struct mvgpu_ctx {
   // splitting (mvgpu_split_communities): labels, peer-exported; the counters reuse q_internal
   DevBuf<int32_t> split_lab;
   SplitPeers spp;
+  // comparing (mvgpu_compare_communities): nothing is peer-exported, every exchange is a collective.  The two
+  // assignments (int32 caller ids), the owned cells and Y-counts, work arrays, and the matches [size|best|overlap|best_size]
+  DevBuf<int32_t> cmp_x, cmp_y, cmp_i0, cmp_i1;
+  DevBuf<unsigned long long> cmp_k0, cmp_k1, cmp_k2, cmp_cell_k, cmp_y_k;
+  DevBuf<uint32_t> cmp_c0, cmp_c1, cmp_c2, cmp_cell_c, cmp_y_c, cmp_b, cmp_hv, cmp_hm;
+  DevBuf<CmpRow> cmp_row0, cmp_row1;
+  DevBuf<long long> cmp_match, cmp_off;
+  DevBuf<int> cmp_n;
   bool run_on_shard = false;           // final_orig holds a run's assignment of the current shard
   bool eval_on_shard = false;          // the q_* arrays describe an evaluation of the current shard
+  bool cmp_on_shard = false;           // cmp_match describes a successful comparison on the current shard's vertices
   // results
   bool unit = true;
   bool f32 = false;                    // shard came through mvgpu_upload_shard32: float-build arithmetic (see mvgpu.h)
@@ -362,6 +373,7 @@ int set_graph(mvgpu_ctx *c, long long nv_global, const int64_t *parts, long long
   if (c->nranks > kMaxRanks) return fail("too many ranks");
   c->have_init = false;                     // an initial assignment belongs to the shard it was given for
   c->run_on_shard = c->eval_on_shard = false;   // so do a run's assignment and an evaluation
+  c->cmp_on_shard = false;                      // and a comparison's matches
   if (nv_global < 0 || lnv < 0 || lne < 0) return fail("negative graph size");
   if (nv_global >= (1LL << 31)) return fail("nv_global >= 2^31: 32-bit community ids would overflow (not supported)");
   if (lne >= (1LL << 32)) return fail("lne >= 2^32 per shard: 32-bit edge offsets would overflow (not supported)");
@@ -1453,6 +1465,260 @@ int split(mvgpu_ctx *c, const int64_t *comm, int64_t *out, mvgpu_split_report *r
   return 0;
 }
 
+// ---- comparing two assignments (DESIGN.md §3.13, compare_gpu.cuh) ---------------------------------------------------
+// Values of a histogram sum to at most N < 2^31, so it has fewer than sqrt(2N) < 65536 distinct positive values: one
+// rank's list (with the value 0 at most once more) always fits this many entries.
+constexpr int kCmpHist = 65536;
+
+// where the keys of a sorted array go: those whose top bits (key >> shift) rank r owns go to r.  Counts and offsets
+// (nranks + 1 of them) both ways.
+struct CmpRoute {
+  std::vector<long long> scount, soff, rcount, roff;
+};
+
+int cmp_route(mvgpu_ctx *c, const unsigned long long *sorted, long long n, int shift, CmpRoute &rt) {
+  const int nr = c->nranks;
+  CmpParts parts;
+  parts.n = nr;
+  for (int r = 0; r <= nr; r++) parts.p[r] = c->parts[r];
+  TRY(c->cmp_off.ensure(nr + 1));
+  k_cmp_bounds<<<1, 32, 0, c->stream>>>(sorted, n, parts, shift, c->cmp_off.p);
+  CK(cudaGetLastError());
+  rt.soff.assign(nr + 1, 0);
+  CK(cudaMemcpyAsync(rt.soff.data(), c->cmp_off.p, sizeof(long long) * (nr + 1), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  rt.scount.assign(nr, 0);
+  for (int r = 0; r < nr; r++) rt.scount[r] = rt.soff[r + 1] - rt.soff[r];
+  std::vector<long long> all(rt.scount);
+  if (nr > 1) {
+    all.resize((size_t)nr * nr);
+    TRY(coll_allgather(c, rt.scount.data(), all.data(), sizeof(long long) * nr));
+  }
+  rt.rcount.assign(nr, 0);
+  rt.roff.assign(nr + 1, 0);
+  for (int r = 0; r < nr; r++) {
+    rt.rcount[r] = all[(size_t)r * nr + c->rank];
+    rt.roff[r + 1] = rt.roff[r] + rt.rcount[r];
+  }
+  return 0;
+}
+
+// send -> recv along rt (back: the reverse way, into an array laid out like the sending side).  The all-to-all moves
+// the other ranks' segments only: this rank's own segment is copied on the device.
+int cmp_move(mvgpu_ctx *c, const void *send, void *recv, const CmpRoute &rt, size_t elem, bool back) {
+  const std::vector<long long> &sc = back ? rt.rcount : rt.scount, &so = back ? rt.roff : rt.soff;
+  const std::vector<long long> &rc = back ? rt.scount : rt.rcount, &ro = back ? rt.soff : rt.roff;
+  const int me = c->rank;
+  if (sc[me])
+    CK(cudaMemcpyAsync((unsigned char *)recv + ro[me] * elem, (const unsigned char *)send + so[me] * elem, sc[me] * elem,
+                       cudaMemcpyDeviceToDevice, c->stream));
+  if (c->nranks > 1) TRY(coll_alltoallv_dev(c, send, sc, so, recv, rc, ro, elem));
+  return 0;
+}
+
+int cmp_read_n(mvgpu_ctx *c, long long &n) {
+  int v = 0;
+  CK(cudaMemcpyAsync(&v, c->cmp_n.p, sizeof v, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  n = v;
+  return 0;
+}
+
+// The n keys in cmp_k0 (unsorted, each below 2^key_bits) -> the distinct keys whose top bits (key >> shift) this rank
+// owns, ascending, in okey, with their number of occurrences over all ranks in ocnt; nout of them.  Every rank sorts and
+// run-length encodes its own keys first, so a key travels to its owner at most once per rank.
+int cmp_reduce(mvgpu_ctx *c, long long n, int key_bits, int shift, DevBuf<unsigned long long> &okey, DevBuf<uint32_t> &ocnt,
+               long long &nout) {
+  cudaStream_t s = c->stream;
+  const bool one = c->nranks == 1;             // one rank owns every key: the local runs are the answer
+  TRY(c->cmp_k1.ensure(n));
+  DevBuf<unsigned long long> &uk = one ? okey : c->cmp_k2;
+  DevBuf<uint32_t> &uc = one ? ocnt : c->cmp_c0;
+  TRY(uk.ensure(n)); TRY(uc.ensure(n));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortKeys(t, tb, c->cmp_k0.p, c->cmp_k1.p, n, 0, key_bits, s); },
+              [&](void *t, size_t &tb) { return cub::DeviceRunLengthEncode::Encode(t, tb, c->cmp_k1.p, uk.p, uc.p, c->cmp_n.p, n, s); }));
+  long long runs = 0;
+  TRY(cmp_read_n(c, runs));
+  if (one) { nout = runs; return 0; }
+  CmpRoute rt;
+  TRY(cmp_route(c, uk.p, runs, shift, rt));
+  const long long m = rt.roff[c->nranks];
+  TRY(c->cmp_k0.ensure(m)); TRY(c->cmp_k1.ensure(m)); TRY(c->cmp_c1.ensure(m)); TRY(c->cmp_c2.ensure(m));
+  TRY(okey.ensure(m)); TRY(ocnt.ensure(m));
+  TRY(cmp_move(c, uk.p, c->cmp_k0.p, rt, sizeof(unsigned long long), false));
+  TRY(cmp_move(c, uc.p, c->cmp_c1.p, rt, sizeof(uint32_t), false));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, c->cmp_k0.p, c->cmp_k1.p, c->cmp_c1.p, c->cmp_c2.p, m, 0, key_bits, s); },
+              [&](void *t, size_t &tb) { return cub::DeviceReduce::ReduceByKey(t, tb, c->cmp_k1.p, okey.p, c->cmp_c2.p, ocnt.p, c->cmp_n.p, CmpSum(), m, s); }));
+  return cmp_read_n(c, nout);
+}
+
+// The histogram of the n values in vals (each <= nv < 2^vbits) as kCmpHist entries value << 32 | multiplicity,
+// ascending value, zero-padded
+int cmp_hist(mvgpu_ctx *c, const uint32_t *vals, long long n, int vbits, std::vector<unsigned long long> &h) {
+  cudaStream_t s = c->stream;
+  TRY(c->cmp_c1.ensure(n)); TRY(c->cmp_hv.ensure(n)); TRY(c->cmp_hm.ensure(n));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortKeys(t, tb, vals, c->cmp_c1.p, n, 0, vbits, s); },
+              [&](void *t, size_t &tb) { return cub::DeviceRunLengthEncode::Encode(t, tb, c->cmp_c1.p, c->cmp_hv.p, c->cmp_hm.p, c->cmp_n.p, n, s); }));
+  long long runs = 0;
+  TRY(cmp_read_n(c, runs));
+  if (runs > kCmpHist) return fail("mvgpu_compare_communities: a histogram with more than 65536 distinct values (counts do not sum to N)");
+  std::vector<uint32_t> v((size_t)runs), m((size_t)runs);
+  if (runs) {
+    CK(cudaMemcpyAsync(v.data(), c->cmp_hv.p, sizeof(uint32_t) * runs, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(m.data(), c->cmp_hm.p, sizeof(uint32_t) * runs, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  h.assign(kCmpHist, 0);
+  for (long long i = 0; i < runs; i++) h[i] = (unsigned long long)v[i] << 32 | m[i];
+  return 0;
+}
+
+// A histogram merged over the ranks: the number of non-zero counts, sum C(k, 2), and S = sum over k > 1, in ascending
+// k, of m * (k * log k).  The merged histogram does not depend on how the vertices are sharded, so neither does S.
+struct CmpHist {
+  long long nonzero = 0;
+  unsigned long long pairs = 0;
+  double s = 0.0;
+};
+
+int cmp_merge(mvgpu_ctx *c, const std::vector<unsigned long long> &mine, CmpHist &out) {
+  std::vector<unsigned long long> all(mine);
+  if (c->nranks > 1) {
+    all.resize((size_t)kCmpHist * c->nranks);
+    TRY(coll_allgather(c, mine.data(), all.data(), sizeof(unsigned long long) * kCmpHist));
+  }
+  std::map<unsigned long long, unsigned long long> h;
+  for (unsigned long long e : all)
+    if (e >> 32) h[e >> 32] += e & 0xffffffffULL;        // value 0 (empty slots, padding) counts nothing
+  out = CmpHist();
+  for (const auto &[k, m] : h) {
+    out.nonzero += (long long)m;
+    out.pairs += m * (k * (k - 1) / 2);
+    if (k > 1) out.s += (double)m * ((double)k * std::log((double)k));
+  }
+  return 0;
+}
+
+// X, Y: this rank's lnv caller ids on the device -> rep's counts (not compare_s) and the matches in cmp_match
+int compare_pass(mvgpu_ctx *c, const int32_t *X, const int32_t *Y, mvgpu_compare_report &rep) {
+  cudaStream_t s = c->stream;
+  const int lnv = (int)c->lnv, nsm = c->num_sms;
+  const long long nv = c->nv_global, base = c->base;
+  int shift = 1, vbits = 1;
+  while ((1LL << shift) < nv) shift++;         // every id < 2^shift
+  while ((1LL << vbits) <= nv) vbits++;        // every count <= nv < 2^vbits
+  TRY(c->cmp_n.ensure(1)); TRY(c->cmp_k0.ensure(lnv));
+  // the cells n_xy of the owned x, and the sizes b_y of the owned y
+  long long ncell = 0, ny = 0, nrows = 0;
+  if (lnv) k_cmp_keys<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, X, Y, shift, c->cmp_k0.p);
+  CK(cudaGetLastError());
+  TRY(cmp_reduce(c, lnv, 2 * shift, shift, c->cmp_cell_k, c->cmp_cell_c, ncell));
+  if (lnv) k_cmp_keys<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, nullptr, Y, 0, c->cmp_k0.p);
+  CK(cudaGetLastError());
+  TRY(cmp_reduce(c, lnv, shift, 0, c->cmp_y_k, c->cmp_y_c, ny));
+  // rows: a_x and the best match of every owned non-empty x (the cells are sorted by x, so its cells are consecutive)
+  TRY(c->cmp_i0.ensure(ncell)); TRY(c->cmp_i1.ensure(ncell)); TRY(c->cmp_row0.ensure(ncell)); TRY(c->cmp_row1.ensure(ncell));
+  TRY(c->cmp_match.ensure(4 * (size_t)lnv));
+  if (lnv) k_cmp_match_init<<<grid_for(lnv, 256, nsm), 256, 0, s>>>(lnv, c->cmp_match.p);
+  if (ncell) k_cmp_cell_rows<<<grid_for(ncell, 256, nsm), 256, 0, s>>>(ncell, c->cmp_cell_k.p, c->cmp_cell_c.p, shift, base, c->cmp_i0.p,
+                                                                         c->cmp_row0.p);
+  CK(cudaGetLastError());
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceReduce::ReduceByKey(t, tb, c->cmp_i0.p, c->cmp_i1.p, c->cmp_row0.p, c->cmp_row1.p,
+                                                                                   c->cmp_n.p, CmpRowOp(), ncell, s); }));
+  TRY(cmp_read_n(c, nrows));
+  TRY(c->cmp_c0.ensure(nrows)); TRY(c->cmp_k0.ensure(nrows)); TRY(c->cmp_k1.ensure(nrows)); TRY(c->cmp_c2.ensure(nrows));
+  // the rows' sizes -> cmp_c0, their best-size requests (best y, asking slot) -> cmp_k0 / cmp_i0
+  if (nrows) k_cmp_rows<<<grid_for(nrows, 256, nsm), 256, 0, s>>>((int)nrows, lnv, c->cmp_i1.p, c->cmp_row1.p, c->cmp_match.p, c->cmp_c0.p,
+                                                                    c->cmp_k0.p, c->cmp_i0.p);
+  TRY(c->cmp_b.ensure(lnv));
+  CK(cudaMemsetAsync(c->cmp_b.p, 0, sizeof(uint32_t) * lnv, s));
+  if (ny) k_cmp_scatter_b<<<grid_for(ny, 256, nsm), 256, 0, s>>>(ny, c->cmp_y_k.p, c->cmp_y_c.p, base, c->cmp_b.p);
+  CK(cudaGetLastError());
+  // best_size: requests sorted by y are grouped by owner; the owner answers b_y in request order
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, c->cmp_k0.p, c->cmp_k1.p, c->cmp_i0.p, c->cmp_i1.p,
+                                                                                    nrows, 0, shift, s); }));
+  CmpRoute rt;
+  TRY(cmp_route(c, c->cmp_k1.p, nrows, 0, rt));
+  const long long nreq = rt.roff[c->nranks];
+  TRY(c->cmp_k2.ensure(nreq)); TRY(c->cmp_c1.ensure(nreq));
+  TRY(cmp_move(c, c->cmp_k1.p, c->cmp_k2.p, rt, sizeof(unsigned long long), false));
+  if (nreq) k_cmp_lookup<<<grid_for(nreq, 256, nsm), 256, 0, s>>>(nreq, c->cmp_k2.p, base, c->cmp_b.p, c->cmp_c1.p);
+  CK(cudaGetLastError());
+  TRY(cmp_move(c, c->cmp_c1.p, c->cmp_c2.p, rt, sizeof(uint32_t), true));
+  if (nrows) k_cmp_best_size<<<grid_for(nrows, 256, nsm), 256, 0, s>>>(nrows, c->cmp_i1.p, c->cmp_c2.p, lnv, c->cmp_match.p);
+  CK(cudaGetLastError());
+  // histograms of the cells, of a and of b, merged over the ranks
+  std::vector<unsigned long long> h;
+  CmpHist hxy, hx, hy;
+  TRY(cmp_hist(c, c->cmp_cell_c.p, ncell, vbits, h)); TRY(cmp_merge(c, h, hxy));
+  TRY(cmp_hist(c, c->cmp_c0.p, nrows, vbits, h)); TRY(cmp_merge(c, h, hx));
+  TRY(cmp_hist(c, c->cmp_y_c.p, ny, vbits, h)); TRY(cmp_merge(c, h, hy));
+  // the report, from the merged integers in a fixed order: the same bits on every rank count
+  const unsigned long long all = (unsigned long long)nv * (unsigned long long)(nv > 0 ? nv - 1 : 0) / 2;
+  rep.vertices = nv; rep.communities_x = hx.nonzero; rep.communities_y = hy.nonzero; rep.cells = hxy.nonzero;
+  rep.pairs_xy = hxy.pairs; rep.pairs_x = hx.pairs; rep.pairs_y = hy.pairs; rep.pairs_all = all;
+  const __int128 A = all, P = hxy.pairs, PX = hx.pairs, PY = hy.pairs;
+  const __int128 num = 2 * (A * P - PX * PY), den = A * (PX + PY) - 2 * PX * PY;
+  rep.ari = den == 0 ? 1.0 : (double)num / (double)den;
+  rep.rand = all == 0 ? 1.0 : (double)(A + 2 * P - PX - PY) / (double)A;
+  const double n = (double)nv;
+  rep.h_x = rep.communities_x <= 1 ? 0.0 : std::log(n) - hx.s / n;
+  rep.h_y = rep.communities_y <= 1 ? 0.0 : std::log(n) - hy.s / n;
+  rep.mi = (rep.communities_x <= 1 || rep.communities_y <= 1) ? 0.0 : std::log(n) + (hxy.s - (hx.s + hy.s)) / n;
+  rep.nmi = (rep.h_x + rep.h_y == 0.0) ? 1.0 : (2.0 * rep.mi) / (rep.h_x + rep.h_y);
+  rep.vi = (rep.h_x + rep.h_y) - 2.0 * rep.mi;
+  return 0;
+}
+
+// collective: every rank passes x or every rank NULL; y is never NULL.  rep and the matches are written only when the
+// call succeeds.  Reads no edge and none of the run's or the evaluation's arrays.
+int compare(mvgpu_ctx *c, const int64_t *x, const int64_t *y, mvgpu_compare_report *rep, const char *caller_err = nullptr) {
+  c->cmp_on_shard = false;                     // a failed call leaves no matches behind
+  TRY(check_ready(c));
+  CK(cudaSetDevice(c->device));
+  const std::string who = "mvgpu_compare_communities";
+  std::string err;
+  std::vector<int32_t> hx, hy;
+  if (caller_err) err = who + ": " + caller_err;
+  else if (c->f32) err = who + ": not for a shard uploaded with mvgpu_upload_shard32";
+  else if (!y) err = who + ": y must not be NULL";
+  else if (!x && !c->run_on_shard) err = who + ": NULL x compares the last mvgpu_louvain result, and there is none on this shard";
+  else {
+    if (x) err = narrow_ids(c, x, who.c_str(), hx);
+    if (err.empty()) err = narrow_ids(c, y, who.c_str(), hy);
+  }
+  // the call's first collective: one rank's finding fails every rank before any data moves
+  if (c->nranks > 1) {
+    TRY(c->scratch.ensure(sizeof(Scalars)));
+    long long hv[2] = {err.empty() ? 0 : 1, x ? 1 : 0};
+    TRY(coll_allreduce_i64(c, hv, 2, false));
+    if (hv[0] && err.empty()) err = who + ": another rank rejected its assignment";
+    if (err.empty() && hv[1] != 0 && hv[1] != c->nranks)
+      err = who + ": ranks disagree on the assignment x: every rank or none must pass NULL";
+  }
+  if (!err.empty()) return fail(err);
+  cudaStream_t s = c->stream;
+  const long long lnv = c->lnv;
+  if (!x) TRY(final_in_caller_order(c));       // one-rank runs leave it unresolved
+  TRY(c->cmp_x.ensure(lnv)); TRY(c->cmp_y.ensure(lnv));
+  if (x && lnv) CK(cudaMemcpyAsync(c->cmp_x.p, hx.data(), sizeof(int32_t) * lnv, cudaMemcpyHostToDevice, s));
+  if (lnv) CK(cudaMemcpyAsync(c->cmp_y.p, hy.data(), sizeof(int32_t) * lnv, cudaMemcpyHostToDevice, s));
+  mvgpu_compare_report r;
+  memset(&r, 0, sizeof r);
+  cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
+  CK(cudaEventRecord(e0, s));
+  TRY(compare_pass(c, x ? c->cmp_x.p : c->final_orig.p, c->cmp_y.p, r));
+  CK(cudaEventRecord(e1, s));
+  CK(cudaEventSynchronize(e1));
+  float ms = 0;
+  CK(cudaEventElapsedTime(&ms, e0, e1));
+  r.compare_s = ms * 1e-3;
+  if (c->nranks > 1) TRY(coll_barrier(c));     // no rank leaves while a peer may still be receiving from it
+  *rep = r;
+  c->cmp_on_shard = true;
+  return 0;
+}
+
 // ---- shard update (DESIGN.md §3.11, merge_gpu.cuh) -------------------------------------------------------------------
 // The shard (n rows, rowptr/edges, lne records) with the sorted deletion keys dkey and the stably sorted insertion keys
 // ikey merged in (iidx: batch index of each sorted insertion, iw: weights in batch order) -> nrow / nedges, *lne_out.
@@ -2044,6 +2310,29 @@ int mv_split_refused(mvgpu_ctx *c, const char *why, mvgpu_split_report *rep) {
   if (!c || !rep || !why) return fail("null argument");
   int64_t none = 0;
   return split(c, nullptr, &none, rep, why);
+}
+
+int mvgpu_compare_communities(mvgpu_ctx *c, const int64_t *x, const int64_t *y, mvgpu_compare_report *rep) {
+  if (!c || !rep) return fail("null argument");
+  return compare(c, x, y, rep);
+}
+
+// Not in mvgpu.h: the Python binding's way into the collective when it cannot build the arrays, as mv_evaluate_refused
+int mv_compare_refused(mvgpu_ctx *c, const char *why, mvgpu_compare_report *rep) {
+  if (!c || !rep || !why) return fail("null argument");
+  return compare(c, nullptr, nullptr, rep, why);
+}
+
+int mvgpu_get_community_matches(mvgpu_ctx *c, int64_t *size, int64_t *best, int64_t *overlap, int64_t *best_size) {
+  if (!c) return fail("null argument");
+  if (!c->cmp_on_shard) return fail("no comparison on this shard yet (mvgpu_compare_communities)");
+  CK(cudaSetDevice(c->device));
+  const size_t n = (size_t)c->lnv;
+  int64_t *dst[4] = {size, best, overlap, best_size};
+  for (int k = 0; k < 4; k++)
+    if (dst[k] && n) CK(cudaMemcpyAsync(dst[k], c->cmp_match.p + k * n, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return 0;
 }
 
 int mvgpu_get_community_stats(mvgpu_ctx *c, int64_t *size, double *volume, double *internal) {

@@ -43,13 +43,25 @@ class SplitReport(ctypes.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class CompareReport(ctypes.Structure):
+    _fields_ = [("vertices", ctypes.c_int64), ("communities_x", ctypes.c_int64), ("communities_y", ctypes.c_int64),
+                ("cells", ctypes.c_int64), ("pairs_xy", ctypes.c_uint64), ("pairs_x", ctypes.c_uint64),
+                ("pairs_y", ctypes.c_uint64), ("pairs_all", ctypes.c_uint64), ("ari", ctypes.c_double),
+                ("rand", ctypes.c_double), ("nmi", ctypes.c_double), ("vi", ctypes.c_double), ("mi", ctypes.c_double),
+                ("h_x", ctypes.c_double), ("h_y", ctypes.c_double), ("compare_s", ctypes.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_destroy", "mvgpu_get_unique_id",
            "mvgpu_comm_init", "mvgpu_upload_shard", "mvgpu_attach_shard_device", "mvgpu_generate_rgg_shard", "mvgpu_generate_rgg_shard_ex",
            "mvgpu_download_shard", "mvgpu_louvain",
            "mvgpu_get_communities", "mvgpu_get_communities_device", "mvgpu_upload_shard32", "mvgpu_louvain32", "mvgpu_get_communities32", "mvgpu_set_option", "mvgpu_get_trace",
            "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method",
            "mvgpu_set_initial_communities", "mvgpu_get_converged", "mvgpu_evaluate_communities",
-           "mvgpu_get_community_stats", "mvgpu_get_compact_communities", "mvgpu_update_shard", "mvgpu_split_communities"]
+           "mvgpu_get_community_stats", "mvgpu_get_compact_communities", "mvgpu_update_shard", "mvgpu_split_communities",
+           "mvgpu_compare_communities", "mvgpu_get_community_matches"]
 
 _lib = None
 
@@ -83,6 +95,9 @@ def lib():
         L.mvgpu_get_community_stats.argtypes = [vp, vp, vp, vp]
         L.mvgpu_split_communities.argtypes = [vp, vp, vp, ctypes.POINTER(SplitReport)]
         L.mv_split_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(SplitReport)]
+        L.mvgpu_compare_communities.argtypes = [vp, vp, vp, ctypes.POINTER(CompareReport)]
+        L.mv_compare_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(CompareReport)]
+        L.mvgpu_get_community_matches.argtypes = [vp, vp, vp, vp, vp]
         L.mvgpu_get_compact_communities.argtypes = [vp, vp]
         L.mvgpu_upload_shard32.argtypes = [vp, ctypes.c_int32, vp, ctypes.c_int32, ctypes.c_int32, vp, vp]
         L.mvgpu_louvain32.argtypes = [vp, ctypes.c_float, ctypes.c_float, ctypes.POINTER(ci), ctypes.POINTER(ctypes.c_float)]
@@ -290,6 +305,34 @@ class LouvainGPU:
         buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
         _ck(lib().mvgpu_split_communities(self._h, buf.ctypes.data, out.ctypes.data, ctypes.byref(rep)))
         return out[:self.lnv], rep.as_dict()
+
+    def compare_communities(self, y, x=None):
+        """Compare two assignments (DESIGN.md §3.13): contingency counts, pair counts, ARI, Rand index, NMI, VI and the
+        entropies, exact and the same on every rank count.  `y` and `x` take the form evaluate() takes; x = None compares
+        what the last louvain() returned.  Collective: every rank passes x or every rank None; a bad id or a wrong
+        length on any rank raises MvgpuError on every rank.  Returns mvgpu_compare_report as a dict; community_matches()
+        then gives the best match of every community of x."""
+        rep = CompareReport()
+        arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.int64) for a in (x, y)]
+        bad = [a for a in arrs if a is not None and (a.ndim != 1 or a.size != self.lnv)]
+        if y is None or bad:
+            # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
+            why = ("y must not be None" if y is None else
+                   f"assignment has {bad[0].size} entries, the shard has lnv = {self.lnv}")
+            _ck(lib().mv_compare_refused(self._h, why.encode(), ctypes.byref(rep)))
+            raise AssertionError("unreachable: a refused comparison fails")
+        bufs = [None if a is None else (a if a.size else np.zeros(1, np.int64)) for a in arrs]   # never NULL for an array
+        _ck(lib().mvgpu_compare_communities(self._h, None if bufs[0] is None else bufs[0].ctypes.data, bufs[1].ctypes.data,
+                                            ctypes.byref(rep)))
+        return rep.as_dict()
+
+    def community_matches(self):
+        """Per community of x in the last compare_communities(): entry s describes community parts[rank] + s.  Returns a
+        dict of int64 arrays `size`, `best`, `overlap` and `best_size`, lnv entries each (best = -1 for an empty x)."""
+        n = max(self.lnv, 1)
+        out = {k: np.zeros(n, np.int64) for k in ("size", "best", "overlap", "best_size")}
+        _ck(lib().mvgpu_get_community_matches(self._h, *[a.ctypes.data for a in out.values()]))
+        return {k: a[:self.lnv] for k, a in out.items()}
 
     def community_stats(self):
         """Per community of the last evaluate(): entry s describes community parts[rank] + s.  Returns a dict of
