@@ -129,6 +129,25 @@ int mvgpu_set_initial_communities(mvgpu_ctx *ctx, const int64_t *comm);
 /* 1 if the last mvgpu_louvain ended on the reference's exit test, 0 if "stop_after" ended it first. */
 int mvgpu_get_converged(mvgpu_ctx *ctx, int *converged);
 
+/* ---- holding vertices in place (DESIGN.md §3.14) ----------------------------------------------------------------------
+ * Movable set M: one byte per vertex, lnv entries in the caller's vertex numbering, nonzero = movable.  In iteration k
+ * with set M_k a vertex outside M_k keeps its community (target = current, no Comm deltas); its counter[0] still counts
+ * toward the iteration's modularity, so the reported modularity, the exit test and the trace keep their definitions.  A
+ * vertex in M_k decides exactly as without a set (same gain, tie order and singleton veto).  Option "frontier": 0
+ * (default) M_k = M in every iteration; 1: M_{k+1} = M_k + { u : a vertex v != u with a stored record v->u has target !=
+ * current in iteration k } (own and ghost tails; u may be owned by another rank); a rejected last iteration does not grow
+ * it.  An all-ones set gives the same bits as no set.
+ * mvgpu_set_movable copies the array at call time (errors are local); it stays in effect for every later mvgpu_louvain on
+ * this shard until NULL clears it (= everything movable) or the next upload / attach / generate; mvgpu_update_shard keeps
+ * it.  In a multi-rank run every rank or none must set one (checked at the start of mvgpu_louvain, which then fails on
+ * every rank).  Not for mvgpu_louvain32. */
+int mvgpu_set_movable(mvgpu_ctx *ctx, const uint8_t *mask);
+/* lnv bytes (0 / 1, caller numbering): the set the next iteration would use -- M_{k+1} after the last accepted iteration k
+ * of the last mvgpu_louvain that ran with a set; before such a run (or after mvgpu_set_movable or mvgpu_update_shard) the
+ * set as given; all ones without a set.  Resuming a run stopped by "stop_after" from (its assignment, this set, lower = its
+ * modularity) with the same "frontier" continues it exactly. */
+int mvgpu_get_movable(mvgpu_ctx *ctx, uint8_t *out);
+
 /* ---- quality of an assignment (DESIGN.md §3.10) ---------------------------------------------------------------------
  * The modularity mvgpu_louvain returns is the reference's mixed quantity: in iteration k the intra-community weight is
  * measured on the assignment the scan read and sum(a_c^2) on the one it wrote.  mvgpu_evaluate_communities gives the
@@ -233,7 +252,8 @@ int mvgpu_get_communities_device(mvgpu_ctx *ctx, const int32_t **d_out);
  * 0 (default) = the 16-byte records as they are), "host_threads" (threads of that host pass, default 8), "stop_after"
  * (0 = off (default); k > 0: end the run successfully after k ACCEPTED iterations: *iters = k, *modularity = prevMod
  * after iteration k -- the `lower` to resume with --, k trace records, mvgpu_get_communities returns the assignment
- * after iteration k; if the exit test fires first the run ends as without it, see mvgpu_get_converged).
+ * after iteration k; if the exit test fires first the run ends as without it, see mvgpu_get_converged), "frontier" (0
+ * (default) / 1: grow the movable set from the vertices that move, see mvgpu_set_movable; no effect without a set).
  * The environment variable MVGPU_OPTIONS="name=value,name=value" presets options for every context of the process. */
 /* In a multi-rank run every rank must set the same options (they change which collectives a run issues). */
 int mvgpu_set_option(mvgpu_ctx *ctx, const char *name, int64_t value);

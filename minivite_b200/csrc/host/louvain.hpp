@@ -33,6 +33,9 @@ struct GpuRankContext {
   std::vector<GraphElem> split_comm;                   // -C: the split assignment of this rank's vertices
   const std::vector<GraphElem> *cmp_comm = nullptr;    // -M: compare the assignment -q would evaluate with this one
   mvgpu_compare_report cmp{};                          // -M: the comparison (global values)
+  const std::vector<unsigned char> *movable = nullptr; // -V: movable set of this rank's vertices (nonzero = movable)
+  bool frontier = false;                               // -F: grow the movable set from the vertices that move
+  std::vector<unsigned char> *movable_out = nullptr;   // -o: the set the next iteration would use (for -V on resume)
 };
 
 [[noreturn]] inline void mv_abort(const std::string &where) {
@@ -70,6 +73,8 @@ inline int mv_env_repeat() {
 inline void mv_apply_warm_start(mvgpu_ctx *ctx, const GpuRankContext &rc) {
   if (rc.init_comm && mvgpu_set_initial_communities(ctx, rc.init_comm->data())) mv_abort("mvgpu_set_initial_communities");
   if (rc.stop_after && mvgpu_set_option(ctx, "stop_after", rc.stop_after)) mv_abort("stop_after");
+  if (rc.movable && mvgpu_set_movable(ctx, rc.movable->data())) mv_abort("mvgpu_set_movable");
+  if (rc.frontier && mvgpu_set_option(ctx, "frontier", 1)) mv_abort("frontier");
 }
 // -C: split `comm` (NULL: the run's result) into rc.split_comm
 inline void mv_split(mvgpu_ctx *ctx, GpuRankContext &rc, const GraphElem *comm, GraphElem lnv) {
@@ -106,6 +111,11 @@ inline void mv_evaluate_run(mvgpu_ctx *ctx, GpuRankContext &rc, GraphElem lnv) {
 }
 // -o: the run's assignment (with -C: its split)
 inline void mv_result(mvgpu_ctx *ctx, GpuRankContext &rc, GraphElem lnv) {
+  if (rc.movable_out) {
+    rc.movable_out->assign(lnv + 1, 1);
+    if (mvgpu_get_movable(ctx, rc.movable_out->data())) mv_abort("mvgpu_get_movable");
+    rc.movable_out->resize(lnv);
+  }
   if (!rc.comm_out) return;
   if (rc.split) { *rc.comm_out = rc.split_comm; return; }
   rc.comm_out->resize(lnv);

@@ -35,7 +35,8 @@
 #include "louvain.hpp"
 #include "rgg.hpp"
 
-static std::string inputFileName, dumpPrefix, initPrefix, evalPrefix, comparePrefix;
+static std::string inputFileName, dumpPrefix, initPrefix, evalPrefix, comparePrefix, movablePrefix;
+static bool frontierGrow = false;
 static int stopAfter = 0;
 static GraphWeight lowerStart = -1.0;
 static int me = 0, nprocs = 1;
@@ -91,7 +92,7 @@ static long long reduce_sum_ll(long long v) {
 
 static void parseCommandLine(const int argc, char *const argv[]) {
   int ret;
-  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:CM:")) != -1) {
+  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:CM:V:F")) != -1) {
     switch (ret) {
       case 'f': inputFileName.assign(optarg); break;
       case 'b': readBalanced = true; break;
@@ -113,6 +114,8 @@ static void parseCommandLine(const int argc, char *const argv[]) {
       case 'E': evalPrefix.assign(optarg); break;
       case 'C': splitComm = true; break;
       case 'M': comparePrefix.assign(optarg); break;
+      case 'V': movablePrefix.assign(optarg); break;
+      case 'F': frontierGrow = true; break;
       default: assert(0 && "Option not recognized!!!"); break;
     }
   }
@@ -232,7 +235,8 @@ int main(int argc, char *argv[]) {
   }
   rc.trace = traceIters;
   std::vector<GraphElem> comm;
-  if (!dumpPrefix.empty()) rc.comm_out = &comm;
+  std::vector<unsigned char> movableOut;
+  if (!dumpPrefix.empty()) { rc.comm_out = &comm; rc.movable_out = &movableOut; }
   if (nprocs > 1) {
     if (me == 0) {
       if (mvgpu_get_unique_id(shm->unique_id)) mv_abort("mvgpu_get_unique_id");
@@ -273,6 +277,22 @@ int main(int argc, char *argv[]) {
     read_assignment("-M", comparePrefix, cmpComm);
     rc.cmp_comm = &cmpComm;
   }
+  // -V: this rank's movable set, PREFIX.<rank> = lnv raw bytes (what -o writes to <o>.mask.<rank>)
+  std::vector<unsigned char> movableIn;
+  if (!movablePrefix.empty()) {
+    const long long want_lnv = deviceGenerate ? (long long)(nvRGG / nprocs) : (long long)g->get_lnv();
+    const std::string fn = movablePrefix + "." + std::to_string(me);
+    FILE *f = fopen(fn.c_str(), "rb");
+    movableIn.assign((size_t)want_lnv + 1, 0);
+    const size_t got = f ? fread(movableIn.data(), 1, movableIn.size(), f) : 0;
+    if (f) fclose(f);
+    const bool ok = f && (long long)got == want_lnv;
+    if (!ok) fprintf(stderr, "[miniVite_b200] -V %s: cannot read %s or it does not hold lnv = %lld bytes\n", movablePrefix.c_str(),
+                     fn.c_str(), want_lnv);
+    if (reduce_sum_ll(ok ? 0 : 1)) abort_all(99);
+    rc.movable = &movableIn;
+  }
+  rc.frontier = frontierGrow;
   rc.stop_after = stopAfter;
   rc.quality = evalQuality;
   rc.split = splitComm;
@@ -329,6 +349,9 @@ int main(int argc, char *argv[]) {
     fwrite(hdr, 8, 2, f);
     fwrite(comm.data(), sizeof(GraphElem), comm.size(), f);
     fclose(f);
+    FILE *fm = fopen((dumpPrefix + ".mask." + std::to_string(me)).c_str(), "wb");
+    fwrite(movableOut.data(), 1, movableOut.size(), fm);
+    fclose(fm);
   }
   if (me == 0 && evalPrefix.empty()) {            // (-E ran no Louvain phase: nothing to report)
     const double avgt = tot_time / nprocs, avgd = dev_time / nprocs;

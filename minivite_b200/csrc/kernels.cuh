@@ -281,9 +281,12 @@ __device__ __forceinline__ void push_move_w(const ScanParams &p, int cc, int bes
 // The trip count of the outer loop is the largest number of distinct neighbour communities among the warp's 32
 // vertices (about 4 after the first iterations) instead of the sum of all lanes' loops.  Sums are accumulated in
 // edge order per community, exactly like k_scan, so the weighted path keeps the reference's rounding.
+// MASKED (DESIGN.md §3.14): `movable` holds one byte per own vertex in internal numbering (read by the MASKED
+// instantiations only, which is why it is a parameter of its own after p); a vertex with movable[v] == 0 leaves after
+// pass 0 -- counter[0] counted, target = current.
 // ----------------------------------------------------------------------------------------------
-template <bool UNIT, bool MULTI, bool TRACE>
-__global__ void __launch_bounds__(kTileV) k_scan_ws(const ScanParams p) {
+template <bool UNIT, bool MULTI, bool TRACE, bool MASKED = false>
+__global__ void __launch_bounds__(kTileV) k_scan_ws(const ScanParams p, const uint8_t *movable) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   int32_t *s_comm = reinterpret_cast<int32_t *>(smem_raw);
   double *s_w = reinterpret_cast<double *>(smem_raw + sizeof(int32_t) * kECap);
@@ -377,6 +380,7 @@ __global__ void __launch_bounds__(kTileV) k_scan_ws(const ScanParams p) {
     if (UNIT) w0 = (double)cnt0;
     const double eix = __dsub_rn(w0, sl), ax = __dsub_rn(cc_deg, vdeg);
     if (d) { if (UNIT) acc_le_u += (unsigned long long)cnt0; else acc_le_d += w0; }
+    if (MASKED && d && !movable[v]) m = 0;                                 // frozen: no candidate, best stays cc
     // pass 1: two distinct neighbour communities per lane per round.  The round's walk counts the community of the
     // first live entry and the first community that differs from it, and compacts everything else to the front, so
     // the live list only ever shrinks and no lane has to skip over already counted entries.
@@ -475,9 +479,10 @@ __global__ void __launch_bounds__(kTileV) k_scan_ws(const ScanParams p) {
 // High-degree vertices (degree > heavy_deg): one CTA per vertex, open-addressing table in HBM
 // scratch (2x degree entries) keyed by neighbour community; same decision rule.  Weighted sums are
 // accumulated with fp64 atomics here (order not fixed: weighted parity is tolerance-based anyway).
+// MASKED: a vertex with movable[v] == 0 still adds its counter[0] share and writes target = current.
 // ----------------------------------------------------------------------------------------------
-template <bool UNIT, bool MULTI, bool TRACE>
-__global__ void __launch_bounds__(256) k_scan_heavy(const ScanParams p) {
+template <bool UNIT, bool MULTI, bool TRACE, bool MASKED = false>
+__global__ void __launch_bounds__(256) k_scan_heavy(const ScanParams p, const uint8_t *movable) {
   const int v = p.heavy_list[blockIdx.x];
   const unsigned long long off = p.heavy_off[blockIdx.x];
   const unsigned int T = (unsigned int)(p.heavy_off[blockIdx.x + 1] - off);   // power of two
@@ -567,6 +572,7 @@ __global__ void __launch_bounds__(256) k_scan_heavy(const ScanParams p) {
       }
     int best = by;
     if (bsz == 1 && cc_size == 1 && label_greater<MULTI>(p, best, lby, cc)) best = cc;
+    if (MASKED && !movable[v]) best = cc;
     if (best != cc) {
       int bo; long long bi;
       locate_impl<MULTI>(p.pt, p.base, p.lnv, best, bo, bi);
@@ -1525,6 +1531,61 @@ __global__ void __launch_bounds__(256) k_split_count(int lnv, const unsigned lon
     if (nonempty) atomicAdd(&agg[0], nonempty);
     if (comps) atomicAdd(&agg[1], comps);
     if (split) atomicAdd(&agg[2], split);
+  }
+}
+
+// ----------------------------------------------------------------------------------------------
+// Movable sets (mvgpu_set_movable, DESIGN.md §3.14).  Both maps run in internal numbering; inv (old -> new local index)
+// is nullptr when this rank was not renumbered.
+// ----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_movable_in(int lnv, const uint8_t *caller, const int32_t *inv, uint8_t *a, uint8_t *b) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < lnv; i += gridDim.x * blockDim.x) {
+    const int j = inv ? inv[i] : i;
+    a[j] = caller[i] != 0;
+    if (b) b[j] = caller[i] != 0;
+  }
+}
+__global__ void __launch_bounds__(256) k_movable_out(int lnv, const uint8_t *mov, const int32_t *inv, uint8_t *caller) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < lnv; i += gridDim.x * blockDim.x) caller[i] = mov[inv ? inv[i] : i];
+}
+
+struct MovPeers {                                   // every rank's next movable set and inv (peer mappings for other ranks)
+  uint8_t *next[kMaxRanks];
+  const int32_t *inv[kMaxRanks];                    // nullptr: that rank was not renumbered
+};
+
+// Frontier growth of one iteration: next := mov | { u : a record v -> u, u != v, with tgt[v] != cur[v] }.  `next`
+// holds a subset of mov on entry (the set of the iteration before; sets only grow), so every store here writes a 1
+// and the stores of several vertices and ranks into one entry need no ordering.  One warp per 32 own vertices; the
+// warp walks each mover's row edge-parallel.  A ghost tail's entry is the owner's, at its internal index.
+__global__ void __launch_bounds__(256) k_frontier_mark(int lnv, const uint32_t *rowptr, const int32_t *tails, const int32_t *cur,
+                                                       const int32_t *tgt, const uint8_t *mov, uint8_t *next,
+                                                       const long long *ghost_gid, PeerTable pt, MovPeers mp) {
+  const int lane = threadIdx.x & 31;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g * 32 < lnv; g += nwarps) {
+    const int v = g * 32 + lane;
+    bool moved = false;
+    if (v < lnv) {
+      if (mov[v] && !next[v]) next[v] = 1;
+      moved = tgt[v] != cur[v];
+    }
+    unsigned int movers = __ballot_sync(0xffffffffu, moved);
+    while (movers) {
+      const int w = g * 32 + __ffs(movers) - 1;
+      movers &= movers - 1;
+      const uint32_t e1 = rowptr[w + 1];
+      for (uint32_t e = rowptr[w] + lane; e < e1; e += 32) {
+        const int t = tails[e];
+        if (t < lnv) {
+          if (t != w) next[t] = 1;
+        } else {
+          int o; long long idx;
+          locate_remote(pt, (int)ghost_gid[t - lnv], o, idx);
+          mp.next[o][mp.inv[o] ? mp.inv[o][idx] : idx] = 1;
+        }
+      }
+    }
   }
 }
 

@@ -107,7 +107,9 @@ struct DevBuf {              // grow-only device buffer (allocations are cached 
   X(inv, c->relabel, need_v, c->peer_inv[r])                        \
   X(q_internal, true, ev ? need_v : 0, c->qp.internal[r])           \
   X(q_rank, true, ev ? need_v + 1 : 0, c->qp.rank[r])                \
-  X(split_lab, true, split ? need_v : 0, c->spp.lab[r])
+  X(split_lab, true, split ? need_v : 0, c->spp.lab[r])             \
+  X(mov_a, c->mov_run && c->opt_frontier, c->mov_run && c->opt_frontier ? need_v : 0, c->peer_mov[0][r]) \
+  X(mov_b, c->mov_run && c->opt_frontier, c->mov_run && c->opt_frontier ? need_v : 0, c->peer_mov[1][r])
 #define MV_COUNT(...) +1
 constexpr int kPeerArrays = 0 MV_EXPORTS(MV_COUNT);
 #undef MV_COUNT
@@ -223,7 +225,7 @@ struct mvgpu_ctx {
   const int32_t *peer_inv[kMaxRanks];  // every rank's inv (old -> new local index) while some rank renumbers: warm-start init only
   Export last_export[kPeerArrays] = {};   // what the last IPC exchange published
   // options
-  int opt_trace = 0, opt_force_weighted = 0, opt_scan_variant = 6, opt_cache_policy = 5, opt_reorder = 2, opt_region = 512, opt_comm_mode = 1, opt_compact_upload = 0, opt_host_threads = 8, opt_first_iter = 1, opt_host_transport = 0;
+  int opt_trace = 0, opt_force_weighted = 0, opt_scan_variant = 6, opt_cache_policy = 5, opt_reorder = 2, opt_region = 512, opt_comm_mode = 1, opt_compact_upload = 0, opt_host_threads = 8, opt_first_iter = 1, opt_host_transport = 0, opt_frontier = 0;
   long long opt_upload_chunk = 4LL << 20;
   long long opt_max_iters = 10000, opt_force_heavy_deg = 0, opt_stop_after = 0;
   // warm start (mvgpu_set_initial_communities): caller-numbered community ids of this shard, until the next graph
@@ -231,6 +233,14 @@ struct mvgpu_ctx {
   bool have_init = false;
   bool warm_run = false;               // the current / last run started from init_comm
   int converged = 1;                   // the last run ended on the exit test (0: stopped by stop_after)
+  // movable set (mvgpu_set_movable, DESIGN.md §3.14): mov_in holds the caller's bytes (caller numbering) until the next
+  // graph; a run keeps M_k in internal numbering in mov_a / mov_b (double-buffered and peer-exported with the frontier
+  // option) and leaves M_{k+1} of its last accepted iteration in mov_out (caller numbering)
+  DevBuf<uint8_t> mov_in, mov_a, mov_b, mov_out;
+  bool have_mov = false;
+  bool mov_run = false;                // the current / last run reads a movable set (the MASKED scan instantiations)
+  bool mov_out_valid = false;          // mov_out describes the last run on this shard
+  uint8_t *peer_mov[2][kMaxRanks];
   // evaluation (mvgpu_evaluate_communities): q_internal and q_rank are peer-exported, the rest stays local
   DevBuf<int32_t> eval_comm;           // the caller's assignment to evaluate (int32 caller ids)
   DevBuf<double> q_internal, q_vol;
@@ -372,6 +382,7 @@ int coll_barrier(mvgpu_ctx *c) {
 int set_graph(mvgpu_ctx *c, long long nv_global, const int64_t *parts, long long lnv, long long lne) {
   if (c->nranks > kMaxRanks) return fail("too many ranks");
   c->have_init = false;                     // an initial assignment belongs to the shard it was given for
+  c->have_mov = c->mov_out_valid = false;   // and so does a movable set
   c->run_on_shard = c->eval_on_shard = false;   // so do a run's assignment and an evaluation
   c->cmp_on_shard = false;                      // and a comparison's matches
   if (nv_global < 0 || lnv < 0 || lne < 0) return fail("negative graph size");
@@ -504,12 +515,13 @@ int setup_peers(mvgpu_ctx *c) {
   return 0;
 }
 
-template <bool UNIT, bool MULTI, bool TRACE>
-int launch_scan_t(mvgpu_ctx *c, const ScanParams &sp, bool first) {
+// MASKED: the run reads a movable set (mov, internal numbering); iteration 1 never takes FIRST then (run_louvain)
+template <bool UNIT, bool MULTI, bool TRACE, bool MASKED>
+int launch_scan_t(mvgpu_ctx *c, const ScanParams &sp, bool first, const uint8_t *mov) {
   const size_t smem = UNIT ? sizeof(int32_t) * 2 * kECap : sizeof(int32_t) * kECap + sizeof(double) * kECap;
   static bool attr_done = false;
   if (!attr_done) {
-    CK(cudaFuncSetAttribute(k_scan_ws<UNIT, MULTI, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(k_scan_ws<UNIT, MULTI, TRACE, MASKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done = true;
   }
   const int tiles = (int)((c->lnv + kTileV - 1) / kTileV);
@@ -518,45 +530,47 @@ int launch_scan_t(mvgpu_ctx *c, const ScanParams &sp, bool first) {
     // stay with k_scan_pw
     static int pq_ctas_per_sm = 0;
     if (!pq_ctas_per_sm) {
-      CK(cudaFuncSetAttribute(k_scan_pq<MULTI, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pq_smem_bytes()));
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pq_ctas_per_sm, k_scan_pq<MULTI, TRACE>, kPwWarps * 32, pq_smem_bytes()));
+      CK(cudaFuncSetAttribute(k_scan_pq<MULTI, TRACE, MASKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pq_smem_bytes()));
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pq_ctas_per_sm, k_scan_pq<MULTI, TRACE, MASKED>, kPwWarps * 32, pq_smem_bytes()));
       if (pq_ctas_per_sm < 1) return fail("k_scan_pq cannot be made resident");
     }
     const int ngroups = (int)((c->lnv + 31) / 32);
     const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, pq_ctas_per_sm * c->num_sms);
-    k_scan_pq<MULTI, TRACE><<<grid, kPwWarps * 32, pq_smem_bytes(), c->stream>>>(sp, ngroups);
+    k_scan_pq<MULTI, TRACE, MASKED><<<grid, kPwWarps * 32, pq_smem_bytes(), c->stream>>>(sp, ngroups, mov);
     c->tm.kernel_launches++; c->tm.scan_launches++;
   } else if (tiles > 0 && c->opt_scan_variant >= 4) {
     // persistent warps, TMA-fed double buffer (scan_pipe.cuh): one CTA slot per resident block, warps stride over groups
     static int pw_ctas_per_sm = 0;
     if (!pw_ctas_per_sm) {
-      CK(cudaFuncSetAttribute(k_scan_pw<UNIT, MULTI, TRACE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes<UNIT>()));
-      CK(cudaFuncSetAttribute(k_scan_pw<UNIT, MULTI, TRACE, UNIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes<UNIT>()));
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pw_ctas_per_sm, k_scan_pw<UNIT, MULTI, TRACE, false>, kPwWarps * 32, pw_smem_bytes<UNIT>()));
+      CK(cudaFuncSetAttribute(k_scan_pw<UNIT, MULTI, TRACE, false, MASKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes<UNIT>()));
+      CK(cudaFuncSetAttribute(k_scan_pw<UNIT, MULTI, TRACE, UNIT && !MASKED, MASKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes<UNIT>()));
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pw_ctas_per_sm, k_scan_pw<UNIT, MULTI, TRACE, false, MASKED>, kPwWarps * 32, pw_smem_bytes<UNIT>()));
       if (pw_ctas_per_sm < 1) return fail("k_scan_pw cannot be made resident");
     }
     const int ngroups = (int)((c->lnv + 31) / 32);
     const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, pw_ctas_per_sm * c->num_sms);
     if (UNIT && first) {
-      k_scan_pw<UNIT, MULTI, TRACE, UNIT><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
+      k_scan_pw<UNIT, MULTI, TRACE, UNIT && !MASKED, MASKED><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups, mov);
       c->lay.first_ran = true;
-    } else k_scan_pw<UNIT, MULTI, TRACE, false><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups);
+    } else k_scan_pw<UNIT, MULTI, TRACE, false, MASKED><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups, mov);
     c->tm.kernel_launches++; c->tm.scan_launches++;
   } else if (tiles > 0) {
-    k_scan_ws<UNIT, MULTI, TRACE><<<tiles, kTileV, UNIT ? sizeof(int32_t) * kECap : smem, c->stream>>>(sp);
+    k_scan_ws<UNIT, MULTI, TRACE, MASKED><<<tiles, kTileV, UNIT ? sizeof(int32_t) * kECap : smem, c->stream>>>(sp, mov);
     c->tm.kernel_launches++; c->tm.scan_launches++;
   }
   if (c->nheavy > 0) {
-    k_scan_heavy<UNIT, MULTI, TRACE><<<(int)c->nheavy, 256, 0, c->stream>>>(sp);
+    k_scan_heavy<UNIT, MULTI, TRACE, MASKED><<<(int)c->nheavy, 256, 0, c->stream>>>(sp, mov);
     c->tm.kernel_launches++; c->tm.scan_launches++;
   }
   CK(cudaGetLastError());
   return 0;
 }
 
-int launch_scan(mvgpu_ctx *c, const ScanParams &sp, bool first) {
+int launch_scan(mvgpu_ctx *c, const ScanParams &sp, bool first, const uint8_t *mov) {
   const bool multi = c->nranks > 1, tr = c->opt_trace != 0;
-#define MV_CASE(U, M, T) if (c->unit == U && multi == M && tr == T) return launch_scan_t<U, M, T>(c, sp, first);
+#define MV_CASE(U, M, T)                                                                                             \
+  if (c->unit == U && multi == M && tr == T)                                                                         \
+    return c->mov_run ? launch_scan_t<U, M, T, true>(c, sp, first, mov) : launch_scan_t<U, M, T, false>(c, sp, first, mov);
   MV_CASE(true, false, false) MV_CASE(true, false, true) MV_CASE(true, true, false) MV_CASE(true, true, true)
   MV_CASE(false, false, false) MV_CASE(false, false, true) MV_CASE(false, true, false) MV_CASE(false, true, true)
 #undef MV_CASE
@@ -662,8 +676,10 @@ int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, 
     bool grow = false;
     for (const Export &e : x) grow = grow || (c->ipc_valid && e.cap && e.cap < e.need);
     const bool assigned = ev ? ev->given : c->warm_run;
-    long long hv[5] = {unit ? 0 : 1, c->lne, err.empty() ? 0 : 1, grow ? 1 : 0, assigned ? 1 : 0};
-    TRY(coll_allreduce_i64(c, hv, 5, false));
+    // [5], [6]: a movable set, and its frontier option (a rank would store into a peer's unexported next set)
+    long long hv[7] = {unit ? 0 : 1, c->lne, err.empty() ? 0 : 1, grow ? 1 : 0, assigned ? 1 : 0, c->mov_run ? 1 : 0,
+                       c->mov_run && c->opt_frontier ? 1 : 0};
+    TRY(coll_allreduce_i64(c, hv, 7, false));
     unit = hv[0] == 0;
     ne_global = hv[1];
     if (hv[2] && err.empty()) err = ev ? "another rank rejected its shard or its assignment" : "another rank rejected its shard";
@@ -671,6 +687,10 @@ int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, 
       err = ev ? (ev->split ? "ranks disagree on the assignment to split: every rank or none must pass NULL"
                             : "ranks disagree on the assignment to evaluate: every rank or none must pass NULL")
                : "ranks disagree on the initial assignment: every rank or none must set one";
+    if (err.empty() && hv[5] != 0 && hv[5] != c->nranks)
+      err = "ranks disagree on the movable set: every rank or none must set one (mvgpu_set_movable)";
+    if (err.empty() && hv[6] != 0 && hv[6] != c->nranks)
+      err = "ranks disagree on the frontier option of the movable set: every rank must set the same value";
     if (hv[3]) {
       close_ipc(c);
       c->peers_ready = false;
@@ -898,6 +918,14 @@ int init_state(mvgpu_ctx *c, const EvalSetup *ev, long long nremote) {
     CK(cudaMemsetAsync(c->q_internal.p, 0, sizeof(double) * lnv, s));
     if (ev->split) TRY(c->split_lab.ensure(lnv));
   }
+  if (c->mov_run) {                           // M_1 = M in internal numbering (both buffers: see k_frontier_mark)
+    TRY(c->mov_a.ensure(lnv)); TRY(c->mov_b.ensure(lnv));
+    if (lnv > 0) {
+      k_movable_in<<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->mov_in.p, c->relabel ? c->inv.p : nullptr, c->mov_a.p,
+                                                           c->opt_frontier ? c->mov_b.p : nullptr);
+      c->tm.kernel_launches++;
+    }
+  }
   if (c->unit)
     k_vertex_init<true><<<grid_for(lnv, 256, nsm), 256, 0, s>>>((int)lnv, c->base, c->a_rowptr, c->a_tails, nullptr, c->comm_a.p,
                                                               c->cdeg.p, c->csize.p, c->upd.p, nullptr, nullptr, nullptr, nullptr,
@@ -972,7 +1000,8 @@ int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
   TRY(c->scratch.ensure(sizeof(Scalars)));
   CK(cudaMemsetAsync(c->scratch.p, 0, sizeof(Scalars), c->stream));
   c->warm_run = ev ? true : c->have_init;
-  Scalars h;                                  // the device scalars after the input pass, then after the 1/(2m) read-back
+  c->mov_run = !ev && c->have_mov;
+  Scalars h;                                 // the device scalars after the input pass, then after the 1/(2m) read-back
   int unit = 0;
   std::string err;
   TRY(input_pass(c, ev, h, unit, err));
@@ -1094,6 +1123,16 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   sp.pt = c->pt;
   sp.loc_cdeg = c->cdeg.p; sp.loc_csize = c->csize.p; sp.loc_upd = c->upd.p; sp.loc_cinfo_w = c->cinfo_w.p;
   sp.loc_usize = c->usize.p; sp.loc_udeg = c->udeg.p; sp.loc_lab = c->relabel ? c->lab.p : nullptr;
+  // movable set: M_k in mov[k_cur]; with the frontier option the scan's movers grow M_{k+1} into the other buffer,
+  // every rank's (mp[b] addresses buffer b on every rank), and an accepted iteration swaps them like cur / tgt
+  uint8_t *mov[2] = {c->mov_a.p, c->mov_b.p};
+  int k_cur = 0;
+  const bool frontier = c->mov_run && c->opt_frontier;
+  MovPeers mp[2];
+  memset(mp, 0, sizeof mp);
+  for (int b = 0; b < 2 && frontier; b++)
+    for (int r = 0; r < c->nranks; r++) { mp[b].next[r] = c->peer_mov[b][r]; mp[b].inv[r] = c->relabel ? c->peer_inv[r] : nullptr; }
+  c->mov_out_valid = false;
   c->last_sp = sp;
 
   const size_t ev_iter0 = ev;
@@ -1120,9 +1159,19 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
       if (numIters == 3) c->scan_kernel = 5;
       else if (numIters >= 5) c->scan_kernel = auto_choice;
     }
-    // (not on a warm run: its communities are not singletons)
-    TRY(launch_scan(c, sp, numIters == 1 && c->simple_sorted && c->opt_first_iter && c->opt_scan_variant >= 4 && !c->f32 && !c->warm_run));
+    // (not on a warm run: its communities are not singletons; not with a movable set: the general reduction gives the
+    // same decisions, and only it has a MASKED instantiation)
+    TRY(launch_scan(c, sp, numIters == 1 && c->simple_sorted && c->opt_first_iter && c->opt_scan_variant >= 4 && !c->f32 && !c->warm_run &&
+                               !c->mov_run, c->mov_run ? mov[k_cur] : nullptr));
     CK(cudaEventRecord(e1, s));
+    if (frontier && c->lnv > 0) {
+      // M_{k+1} from this scan's movers; the stores into peers' sets are ordered before their next scan by the barrier
+      // below, like the remote Comm deltas
+      k_frontier_mark<<<grid_for((c->lnv + 7) / 8, 256, c->num_sms), 256, 0, s>>>((int)c->lnv, c->a_rowptr, c->a_tails, cur, tgt, mov[k_cur],
+                                                                                 mov[k_cur ^ 1], c->ghost_gid.p, c->pt, mp[k_cur ^ 1]);
+      c->tm.kernel_launches++;
+      CK(cudaGetLastError());
+    }
     const bool p2p = c->nranks > 1 && c->opt_comm_mode == 1;
     if (c->nranks > 1) {
       // ghost values of the NEW assignment go into the ghost tail of every peer's tgt array; then "every scan has
@@ -1175,6 +1224,7 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
     prevMod = currMod;
     if (prevMod < lower) prevMod = lower;                      // dspl.hpp:1404-1406
     std::swap(cur, tgt);                                       // rotation (dspl.hpp:1408-1422) is a pointer swap
+    if (frontier) k_cur ^= 1;                                  // M_{k+1} only for an accepted iteration
     if (c->opt_stop_after > 0 && numIters == c->opt_stop_after) { c->converged = 0; break; }   // checkpoint: resume with lower = prevMod
   }
   cudaEvent_t e_end = get_event(c, ev++);
@@ -1182,6 +1232,14 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   c->d_final = cur;
   c->final_ready = false;
   c->run_on_shard = true;
+  if (c->mov_run) {                                            // M_{k+1} in caller numbering, outside the timed region
+    TRY(c->mov_out.ensure(c->lnv));
+    if (c->lnv > 0) {
+      k_movable_out<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, s>>>((int)c->lnv, mov[k_cur], c->relabel ? c->inv.p : nullptr, c->mov_out.p);
+      CK(cudaGetLastError());
+    }
+    c->mov_out_valid = true;
+  }
   if (c->nranks > 1) {
     // the assignment in the caller's numbering needs the label arrays of the PEERS (a community may be owned by another
     // rank): resolve it now, while every rank is still inside this call, and leave together -- afterwards a rank may
@@ -2263,7 +2321,8 @@ int mvgpu_update_shard(mvgpu_ctx *c, int64_t n_del, const int64_t *del_src, cons
   ed.swap(nedges);
   c->lne = lne2;
   set_source(c, rp.p, ed.p, nullptr, false, 0.0, 0);
-  c->run_on_shard = c->eval_on_shard = false;   // the initial assignment stays: parts and lnv have not changed
+  c->run_on_shard = c->eval_on_shard = false;   // the initial assignment and the movable set stay: parts and lnv have not changed
+  c->mov_out_valid = false;
   c->peers_ready = false;                       // ghost lists and receive offsets change with the records, on every rank
   if (lne_out) *lne_out = lne2;
   return 0;
@@ -2285,6 +2344,38 @@ int mvgpu_set_initial_communities(mvgpu_ctx *c, const int64_t *comm) {
   TRY(c->init_comm.ensure(c->lnv));
   if (c->lnv) CK(cudaMemcpy(c->init_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice));
   c->have_init = true;
+  return 0;
+}
+
+int mvgpu_set_movable(mvgpu_ctx *c, const uint8_t *mask) {
+  if (!c) return fail("null argument");
+  c->mov_out_valid = false;
+  c->peers_ready = false;          // a masked run with the frontier option exports two more arrays
+  if (!mask) { c->have_mov = false; return 0; }
+  if (!c->have_graph) return fail("mvgpu_set_movable: no shard yet (upload, attach or generate one first)");
+  CK(cudaSetDevice(c->device));
+  TRY(c->mov_in.ensure(c->lnv));
+  if (c->lnv) {                                // on the context's stream, behind any run still reading mov_in
+    CK(cudaMemcpyAsync(c->mov_in.p, mask, c->lnv, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+  }
+  c->have_mov = true;
+  return 0;
+}
+
+int mvgpu_get_movable(mvgpu_ctx *c, uint8_t *out) {
+  if (!c || !out) return fail("null argument");
+  if (!c->have_graph) return fail("mvgpu_get_movable: no shard yet (upload, attach or generate one first)");
+  if (c->lnv == 0) return 0;
+  CK(cudaSetDevice(c->device));
+  // on the context's stream: the run leaves k_movable_out queued behind its end event (and c->stream does not
+  // synchronise with the legacy default stream)
+  if (c->mov_out_valid || c->have_mov) {
+    CK(cudaMemcpyAsync(out, c->mov_out_valid ? c->mov_out.p : c->mov_in.p, c->lnv, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    if (!c->mov_out_valid)                     // the set as given, as 0 / 1
+      for (long long i = 0; i < c->lnv; i++) out[i] = out[i] != 0;
+  } else memset(out, 1, (size_t)c->lnv);
   return 0;
 }
 
@@ -2430,6 +2521,7 @@ int mvgpu_set_option(mvgpu_ctx *c, const char *name, int64_t value) {
   else if (n == "compact_upload") c->opt_compact_upload = (int)value;
   else if (n == "host_threads") c->opt_host_threads = (int)value;
   else if (n == "first_iter") c->opt_first_iter = value != 0;
+  else if (n == "frontier") { if (value != 0 && value != 1) return fail("frontier must be 0 or 1"); c->opt_frontier = (int)value; }
   else if (n == "stop_after") { if (value < 0) return fail("stop_after < 0"); c->opt_stop_after = value; }
   else if (n == "upload_chunk") { if (value < 256 || (value & 3)) return fail("upload_chunk must be a multiple of 4, >= 256"); c->opt_upload_chunk = value; }
   else if (n == "host_transport") {
@@ -2542,6 +2634,7 @@ int mvgpu_louvain32(mvgpu_ctx *c, float lower, float thresh, int *iters, float *
   if (!c || !iters || !modularity) return fail("null argument");
   if (!c->f32) return fail("mvgpu_louvain32 needs a shard uploaded with mvgpu_upload_shard32");
   if (c->have_init || c->opt_stop_after) return fail("mvgpu_louvain32 supports neither an initial assignment nor stop_after");
+  if (c->have_mov) return fail("mvgpu_louvain32 does not support a movable set (mvgpu_set_movable)");
   double mod = 0.0;
   TRY(run_louvain(c, (double)lower, (double)thresh, iters, &mod));
   *modularity = (float)mod;

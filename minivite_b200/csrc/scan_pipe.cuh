@@ -77,10 +77,12 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-template <bool UNIT, bool MULTI, bool TRACE, bool FIRST>
+// MASKED (DESIGN.md §3.14): a vertex with movable[v] == 0 skips pass 1 and stays (counter[0] still counted).
+template <bool UNIT, bool MULTI, bool TRACE, bool FIRST, bool MASKED = false>
 __global__ void __launch_bounds__(kPwWarps * 32, UNIT ? MV_PW_RES_WARPS / kPwWarps : 24 / kPwWarps)
-k_scan_pw(const ScanParams p, int ngroups) {
+k_scan_pw(const ScanParams p, int ngroups, const uint8_t *movable) {
   static_assert(!FIRST || UNIT, "the first-iteration reduction exists for the unit-weight path only");
+  static_assert(!(FIRST && MASKED), "a masked run takes the general reduction in iteration 1");
   constexpr int CAP = PwCap<UNIT>::value;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -295,6 +297,7 @@ k_scan_pw(const ScanParams p, int ngroups) {
       if (UNIT) w0 = (double)cnt0;
       const double eix = __dsub_rn(w0, sl), ax = __dsub_rn(cc_deg, vdeg);
       if (d) { if (UNIT) acc_le_u += (unsigned long long)cnt0; else acc_le_d += w0; }
+      if (MASKED && d && !movable[v]) m = 0;                                 // frozen: no candidate, best stays cc
       // ---- pass 1: two distinct neighbour communities per lane per round (see k_scan_ws)
       double bg = 0.0;
       for (;;) {

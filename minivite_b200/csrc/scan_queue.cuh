@@ -40,8 +40,10 @@ constexpr int kPqCap = MV_WCAP_UNIT;   // edges in the (single) tail buffer
 constexpr int kPqWarpBytes = ((kPqCap * 4 + 3 * kPwRows * 4 + kQSlots * kQEnt * 4 + kQSlots * 16 + 4 * 8) + 127) / 128 * 128;
 constexpr size_t pq_smem_bytes() { return (size_t)kPwWarps * kPqWarpBytes; }
 
-template <bool MULTI, bool TRACE>
-__global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_scan_pq(const ScanParams p, int ngroups) {
+// MASKED (DESIGN.md §3.14): a vertex with movable[v] == 0 is treated like one whose bound is <= 0: never hard, never
+// parked, it stays.
+template <bool MULTI, bool TRACE, bool MASKED = false>
+__global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_scan_pq(const ScanParams p, int ngroups, const uint8_t *movable) {
   constexpr int CAP = kPqCap;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -253,7 +255,8 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
       // ---- can any candidate beat maxGain = 0?  (see the header: exact upper bound on curGain)
       const double gB = __dmul_rn(__dmul_rn(__dmul_rn(2.0, vdeg), ax), p.constant);
       const double bound = __dadd_rn(__dmul_rn(2.0, __dsub_rn((double)m, eix)), gB);
-      const bool hard = m > 0 && (p.f32 || !(bound <= 0.0));    // the bounds are derived for the double-precision gain
+      const bool hard = m > 0 && (p.f32 || !(bound <= 0.0))     // the bounds are derived for the double-precision gain
+                        && (!MASKED || movable[v]);
       const uint32_t hmask = __ballot_sync(0xffffffffu, hard);
       const bool in_place = __any_sync(0xffffffffu, hard && m > kQEnt);
       if (in_place) {

@@ -61,7 +61,7 @@ EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_dest
            "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method",
            "mvgpu_set_initial_communities", "mvgpu_get_converged", "mvgpu_evaluate_communities",
            "mvgpu_get_community_stats", "mvgpu_get_compact_communities", "mvgpu_update_shard", "mvgpu_split_communities",
-           "mvgpu_compare_communities", "mvgpu_get_community_matches"]
+           "mvgpu_compare_communities", "mvgpu_get_community_matches", "mvgpu_set_movable", "mvgpu_get_movable"]
 
 _lib = None
 
@@ -90,6 +90,8 @@ def lib():
         L.mvgpu_get_communities.argtypes = [vp, vp]
         L.mvgpu_set_initial_communities.argtypes = [vp, vp]
         L.mvgpu_get_converged.argtypes = [vp, ctypes.POINTER(ci)]
+        L.mvgpu_set_movable.argtypes = [vp, vp]
+        L.mvgpu_get_movable.argtypes = [vp, vp]
         L.mvgpu_evaluate_communities.argtypes = [vp, vp, ctypes.POINTER(Quality)]
         L.mv_evaluate_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(Quality)]
         L.mvgpu_get_community_stats.argtypes = [vp, vp, vp, vp]
@@ -145,6 +147,7 @@ class LouvainGPU:
         self.rank, self.nranks, self.device = rank, nranks, device
         _ck(lib().mvgpu_create(ctypes.byref(self._h), device, rank, nranks))
         self.lnv = 0
+        self.base = 0                # global id of this rank's first vertex
         self._keep = None
 
     def comm_init(self, unique_id: bytes):
@@ -161,7 +164,7 @@ class LouvainGPU:
         assert int(rowptr[-1]) == lne
         _ck(lib().mvgpu_upload_shard(self._h, int(nv_global), parts.ctypes.data, lnv, lne, rowptr.ctypes.data,
                                      edges.ctypes.data if lne else None))
-        self.lnv = lnv
+        self.lnv, self.base = lnv, int(parts[self.rank])
 
     # ---- the reference's USE_32_BIT_GRAPH build: int32 ids, float weights, float results (include/mvgpu.h)
     def upload32(self, nv_global, parts, rowptr, edges):
@@ -173,7 +176,7 @@ class LouvainGPU:
         assert int(rowptr[-1]) == lne
         _ck(lib().mvgpu_upload_shard32(self._h, int(nv_global), parts.ctypes.data, lnv, lne, rowptr.ctypes.data,
                                        edges.ctypes.data if lne else None))
-        self.lnv = lnv
+        self.lnv, self.base = lnv, int(parts[self.rank])
 
     def louvain32(self, lower=-1.0, thresh=1.0e-6):
         iters = ctypes.c_int(0)
@@ -191,7 +194,7 @@ class LouvainGPU:
         parts = np.ascontiguousarray(parts, dtype=np.int64)
         _ck(lib().mvgpu_attach_shard_device(self._h, int(nv_global), parts.ctypes.data, int(lnv), int(lne),
                                             ctypes.c_void_p(d_rowptr_ptr), ctypes.c_void_p(d_edges_ptr)))
-        self.lnv = int(lnv)
+        self.lnv, self.base = int(lnv), int(parts[self.rank])
         self._keep = keepalive
 
     def generate_rgg(self, nv_global, unit_weight=True, lcg=False, random_edge_percent=0.0):
@@ -201,6 +204,7 @@ class LouvainGPU:
         _ck(lib().mvgpu_generate_rgg_shard_ex(self._h, int(nv_global), int(bool(unit_weight)), int(bool(lcg)),
                                               float(random_edge_percent), ctypes.byref(lne)))
         self.lnv = int(nv_global) // self.nranks
+        self.base = self.rank * self.lnv
         self._lne = lne.value
         return lne.value
 
@@ -259,6 +263,43 @@ class LouvainGPU:
             raise ValueError(f"initial assignment has {comm.size} entries, the shard has lnv = {self.lnv}")
         buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
         _ck(lib().mvgpu_set_initial_communities(self._h, buf.ctypes.data))
+
+    def set_movable(self, mask):
+        """Hold vertices in place (DESIGN.md §3.14): every later louvain() on this shard lets only the vertices with a
+        nonzero byte in `mask` (lnv entries, caller's vertex numbering) move; with the option frontier = 1 the set grows
+        from the vertices that move.  None clears it (everything movable); a new upload / attach / generate clears it too,
+        update_shard keeps it.  With several ranks every rank or none must set one."""
+        if mask is None:
+            _ck(lib().mvgpu_set_movable(self._h, None))
+            return
+        mask = np.ascontiguousarray(mask)
+        if mask.ndim != 1 or mask.size != self.lnv:
+            raise ValueError(f"movable set has {mask.size} entries, the shard has lnv = {self.lnv}")
+        buf = (mask != 0).astype(np.uint8) if mask.dtype != np.uint8 else mask
+        if not buf.size:
+            buf = np.zeros(1, np.uint8)                          # an empty shard still passes a non-NULL array
+        _ck(lib().mvgpu_set_movable(self._h, buf.ctypes.data))
+
+    def movable(self):
+        """The set the next iteration would use (uint8 0 / 1, lnv entries): after a run with a set, the set after its last
+        accepted iteration -- resume a stop_after checkpoint with it; otherwise the set as given, all ones without one."""
+        out = np.zeros(max(self.lnv, 1), np.uint8)
+        _ck(lib().mvgpu_get_movable(self._h, out.ctypes.data))
+        return out[:self.lnv]
+
+    def movable_from_batch(self, delete=None, insert=None):
+        """The lnv mask (uint8) of this rank's `src` endpoints of an update_shard batch: delete = (src, dst), insert =
+        (src, dst, w) as update_shard takes them.  The caller gives both directions of every edge, so every endpoint is
+        covered on its owner without communication.  Endpoints outside this rank raise ValueError."""
+        mask = np.zeros(self.lnv, np.uint8)
+        for t in (delete, insert):
+            if t is None:
+                continue
+            src = np.ascontiguousarray(t[0], dtype=np.int64).reshape(-1) - self.base
+            if src.size and (src.min() < 0 or src.max() >= self.lnv):
+                raise ValueError("batch src outside this rank's vertices")
+            mask[src] = 1
+        return mask
 
     def converged(self):
         """True if the last louvain() ended on the exit test, False if the stop_after option ended it first."""
