@@ -26,6 +26,22 @@
  * integer (dspl.hpp:285), clusterWeight is measured before the moves and the
  * degree term after them (407-456), the returned modularity is that of the last
  * ACCEPTED iteration while `iters` counts the rejected one too (1401-1440).
+ *
+ * Three extensions, each off by default (init_comm = NULL, stop_after = 0, movable = NULL gives the pinned loop above,
+ * operation for operation); tests/test_oracle.py and tests/test_movable_oracle.py hold them to the pinned path:
+ *   init_comm   (warm start, DESIGN.md §3.9) every shard's starting currComm, global community ids in [0, nv).
+ *               localCinfo is then the aggregate of that assignment: sizes counted and degrees summed in global vertex
+ *               order.
+ *   stop_after  > 0: end the run after that many ACCEPTED iterations; currComm is then the assignment after the last one
+ *               and the return value its clamped prevMod (the `lower` to resume with).  *converged_out (may be NULL)
+ *               is 0 then, and 1 when the reference's exit test ended the run.
+ *   movable     (movable set, DESIGN.md §3.14) per shard, one byte per vertex, nonzero = movable.  A vertex outside M_k
+ *               keeps its community in iteration k (targetComm = currComm, no Comm deltas); its counter[0] still enters
+ *               clusterWeight, so the modularity keeps its definition.
+ *   frontier    1: M_{k+1} = M_k + { u : a vertex v != u with a record v->u has targetComm != currComm in iteration k },
+ *               taken over only when iteration k is accepted; 0: M_k = M.  Without a movable set it changes nothing.
+ *   movable_out (may be NULL) per shard: the set the next iteration would use when the run ends (all ones without a
+ *               movable set).
  */
 #include <math.h>
 #include <stdint.h>
@@ -161,13 +177,26 @@ static GraphElem get_max_index(const GraphElem *clkeys, const GraphWeight *count
  * (lnv+1 entries), edges[r] carry GLOBAL tails, exactly the arrays of a reference Graph.
  * Outputs: *iters_out (dspl.hpp:1430), returns prevMod (dspl.hpp:1440); comm_out[r] (may be NULL)
  * receives currComm of shard r at exit; trace[0..min(iters,max_trace)) the per-iteration records;
- * *constant_out = 1/(2m).  Returns NaN on allocation failure. */
+ * *constant_out = 1/(2m).  Returns NaN on allocation failure.  init_comm, stop_after, converged_out, movable,
+ * frontier and movable_out are the extensions of the header. */
 double mvo_louvain(int nranks, const int64_t *parts, const int64_t *const *rowptr, const void *const *edges,
                    double lower, double thresh, int *iters_out, int64_t *const *comm_out,
-                   MvoIterTrace *trace, int max_trace, double *constant_out) {
+                   MvoIterTrace *trace, int max_trace, double *constant_out,
+                   const int64_t *const *init_comm, int stop_after, int *converged_out,
+                   const uint8_t *const *movable, int frontier, uint8_t *const *movable_out) {
   Rank *RK = (Rank *)calloc((size_t)nranks, sizeof(Rank));
   GraphElem nv_global = parts[nranks];
   GraphElem maxdeg = 0;
+  uint8_t **M = NULL, **Mn = NULL;   /* M_k, and M_{k+1} while iteration k runs; NULL = every vertex movable */
+  if (movable) {
+    M = (uint8_t **)calloc((size_t)nranks, sizeof(uint8_t *));
+    Mn = (uint8_t **)calloc((size_t)nranks, sizeof(uint8_t *));
+    for (int r = 0; r < nranks; r++) {
+      const GraphElem nv = parts[r + 1] - parts[r];
+      M[r] = (uint8_t *)malloc((size_t)nv + 1); Mn[r] = (uint8_t *)malloc((size_t)nv + 1);
+      for (GraphElem i = 0; i < nv; i++) M[r][i] = (movable[r][i] != 0);
+    }
+  }
 
   /* ---- distInitLouvain, dspl.hpp:151-172 ---- */
   GraphWeight totalEdgeWeightTwice = 0.0;
@@ -195,6 +224,20 @@ double mvo_louvain(int nranks, const int64_t *parts, const int64_t *const *rowpt
     for (GraphElem i = 0; i < nv; i++) localWeight += R->vDegree[i];   /* dspl.hpp:122-123 */
     totalEdgeWeightTwice += localWeight;                                  /* Allreduce, rank order */
     for (GraphElem i = 0; i < nv; i++) { R->pastComm[i] = i + R->base; R->currComm[i] = i + R->base; }  /* 132-149 */
+  }
+  if (init_comm) {                                         /* warm start: the aggregate of the given assignment */
+    for (int r = 0; r < nranks; r++)
+      for (GraphElem i = 0; i < RK[r].nv; i++) { RK[r].localCinfo[i].size = 0; RK[r].localCinfo[i].degree = 0.0; }
+    for (int r = 0; r < nranks; r++) {
+      Rank *R = &RK[r];
+      for (GraphElem i = 0; i < R->nv; i++) {
+        const GraphElem c = init_comm[r][i];
+        const int o = get_owner(parts, nranks, c);
+        R->pastComm[i] = c; R->currComm[i] = c;
+        RK[o].localCinfo[c - RK[o].base].size++;
+        RK[o].localCinfo[c - RK[o].base].degree += R->vDegree[i];
+      }
+    }
   }
   const GraphWeight constantForSecondTerm = 1.0 / totalEdgeWeightTwice;    /* dspl.hpp:129 */
   if (constant_out) *constant_out = constantForSecondTerm;
@@ -226,7 +269,7 @@ double mvo_louvain(int nranks, const int64_t *parts, const int64_t *const *rowpt
   Map clmap; map_init(&clmap, maxdeg + 2);   /* never grows: at most maxdeg+1 keys per vertex */
 
   GraphWeight prevMod = lower, currMod = -1.0;
-  int numIters = 0;
+  int numIters = 0, converged = 1;
 
   for (;;) {                                               /* dspl.hpp:1338 */
     numIters++;
@@ -289,6 +332,7 @@ double mvo_louvain(int nranks, const int64_t *parts, const int64_t *const *rowpt
           for (int64_t k = 0; k < nclus; k++) clmap.keys[clpos[k]] = -1;   /* reset scratch map */
           clmap.n = 0;
         } else localTarget = cc;
+        if (M && !M[r][i]) localTarget = cc;               /* held in place: counter[0] above still counted */
         if (localTarget >= base && localTarget < bound) targetCommIsLocal = 1;
         if (localTarget != cc && localTarget != -1) {      /* the four cases of 331-399 */
           if (targetCommIsLocal) { R->localCupdate[localTarget - base].degree += R->vDegree[i]; R->localCupdate[localTarget - base].size++; }
@@ -301,6 +345,22 @@ double mvo_louvain(int nranks, const int64_t *parts, const int64_t *const *rowpt
       for (GraphElem i = 0; i < nv; i++) {                 /* distUpdateLocalCinfo, 458-471 */
         R->localCinfo[i].size += R->localCupdate[i].size;
         R->localCinfo[i].degree += R->localCupdate[i].degree;
+      }
+    }
+    /* ---- frontier: M_{k+1} = M_k + the tails of the movers' records (own or remote, self loops excluded) ---- */
+    if (M) {
+      for (int r = 0; r < nranks; r++) memcpy(Mn[r], M[r], (size_t)RK[r].nv);
+      for (int r = 0; r < nranks && frontier; r++) {
+        Rank *R = &RK[r];
+        for (GraphElem i = 0; i < R->nv; i++) {
+          if (R->targetComm[i] == R->currComm[i]) continue;
+          for (GraphElem j = R->rowptr[i]; j < R->rowptr[i + 1]; j++) {
+            const GraphElem u = R->edges[j].tail;
+            if (u == i + R->base) continue;
+            const int o = get_owner(parts, nranks, u);
+            Mn[o][u - RK[o].base] = 1;
+          }
+        }
       }
     }
     /* ---- updateRemoteCommunities, dspl.hpp:978-1103: owner adds deltas in source-rank order,
@@ -357,18 +417,27 @@ double mvo_louvain(int nranks, const int64_t *parts, const int64_t *const *rowpt
       Rank *R = &RK[r];
       GraphElem *tmp = R->pastComm; R->pastComm = R->currComm; R->currComm = R->targetComm; R->targetComm = tmp;
     }
+    if (M)                                                 /* accepted: M_{k+1} */
+      for (int r = 0; r < nranks; r++) { uint8_t *t = M[r]; M[r] = Mn[r]; Mn[r] = t; }
+    if (stop_after > 0 && numIters == stop_after) { converged = 0; break; }
   }
+  if (converged_out) *converged_out = converged;
 
   *iters_out = numIters;
   for (int r = 0; r < nranks; r++) {
     Rank *R = &RK[r];
     if (comm_out && comm_out[r]) memcpy(comm_out[r], R->currComm, sizeof(GraphElem) * (size_t)R->nv);
+    if (movable_out && movable_out[r]) {
+      if (M) memcpy(movable_out[r], M[r], (size_t)R->nv);
+      else memset(movable_out[r], 1, (size_t)R->nv);
+    }
+    if (M) { free(M[r]); free(Mn[r]); }
     free(R->pastComm); free(R->currComm); free(R->targetComm); free(R->vDegree); free(R->clusterWeight);
     free(R->localCinfo); free(R->localCupdate); free(R->rvdata); free(R->rcomm_val);
     map_free(&R->remoteComm); map_free(&R->remoteC);
     free(R->remoteCkey); free(R->remoteCinfo); free(R->remoteCupdate);
   }
-  map_free(&clmap); free(clkeys); free(clpos); free(counter); free(RK);
+  map_free(&clmap); free(clkeys); free(clpos); free(counter); free(RK); free(M); free(Mn);
   (void)nv_global;
   return prevMod;                                          /* dspl.hpp:1440 */
 }

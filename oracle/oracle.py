@@ -41,13 +41,14 @@ _lib = None
 def _load():
     global _lib
     if _lib is None:
-        if not os.path.exists(LIB):
+        if not os.path.exists(LIB) or os.path.getmtime(LIB) < os.path.getmtime(SRC):
             build()
         L = ctypes.CDLL(LIB)
+        vp = ctypes.c_void_p
         L.mvo_louvain.restype = ctypes.c_double
-        L.mvo_louvain.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_double,
-                                  ctypes.c_double, ctypes.POINTER(ctypes.c_int), ctypes.c_void_p, ctypes.c_void_p,
-                                  ctypes.c_int, ctypes.POINTER(ctypes.c_double)]
+        L.mvo_louvain.argtypes = [ctypes.c_int, vp, vp, vp, ctypes.c_double, ctypes.c_double, ctypes.POINTER(ctypes.c_int),
+                                  vp, vp, ctypes.c_int, ctypes.POINTER(ctypes.c_double), vp, ctypes.c_int,
+                                  ctypes.POINTER(ctypes.c_int), vp, ctypes.c_int, vp]
         L.mvo_comm_hash.restype = ctypes.c_uint64
         L.mvo_comm_hash.argtypes = [ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p]
         _lib = L
@@ -59,35 +60,53 @@ def comm_hash(base, comm):
     return int(_load().mvo_comm_hash(int(base), len(comm), comm.ctypes.data))
 
 
-def louvain(parts, rowptrs, edge_lists, lower=-1.0, thresh=1.0e-6, max_trace=512):
-    """Run the C restatement on shards (parts[r]..parts[r+1]); returns a dict with modularity, iters,
-    trace (structured array), comm (list of int64 arrays, currComm at exit), constant, chash_final."""
+def louvain(parts, rowptrs, edge_lists, lower=-1.0, thresh=1.0e-6, max_trace=512, init_comm=None, stop_after=0,
+            movable=None, frontier=0):
+    """Run the C restatement on shards (parts[r]..parts[r+1]).  init_comm: per-shard starting assignments in global
+    community ids (None = singletons); stop_after > 0: stop after that many accepted iterations; movable: per-shard byte
+    masks, nonzero = movable (None = every vertex movable); frontier 0 / 1 (louvain_oracle.c's header).  Returns a dict
+    with modularity, iters, trace (structured array), comm (list of int64 arrays, currComm at exit), constant,
+    chash_final, converged (False when stop_after ended the run) and movable (per shard, the set, uint8 0 / 1, the next
+    iteration would use)."""
     L = _load()
     n = len(rowptrs)
     parts = np.ascontiguousarray(parts, dtype=np.int64)
     assert len(parts) == n + 1
+    sizes = [int(parts[r + 1] - parts[r]) for r in range(n)]
     rps = [np.ascontiguousarray(r, dtype=np.int64) for r in rowptrs]
-    eds = []
-    for e in edge_lists:
-        e = np.ascontiguousarray(e)
-        assert e.dtype.itemsize == 16
-        eds.append(e)
-    comm = [np.zeros(int(parts[r + 1] - parts[r]), dtype=np.int64) for r in range(n)]
+    eds = [np.ascontiguousarray(e) for e in edge_lists]
+    assert all(e.dtype.itemsize == 16 for e in eds)
+    comm = [np.zeros(s, dtype=np.int64) for s in sizes]
+    mov_out = [np.zeros(s, dtype=np.uint8) for s in sizes]
     PtrArr = ctypes.c_void_p * n
-    rp_ptrs = PtrArr(*[r.ctypes.data for r in rps])
-    ed_ptrs = PtrArr(*[e.ctypes.data if len(e) else None for e in eds])
-    cm_ptrs = PtrArr(*[c.ctypes.data if len(c) else None for c in comm])
+
+    def arr(xs):
+        return ctypes.cast(PtrArr(*[x.ctypes.data if len(x) else None for x in xs]), ctypes.c_void_p)
+    init = mov = None
+    if init_comm is not None:
+        assert len(init_comm) == n
+        init = [np.ascontiguousarray(c, dtype=np.int64) for c in init_comm]
+        for r in range(n):
+            assert len(init[r]) == sizes[r]
+            assert len(init[r]) == 0 or (init[r].min() >= 0 and init[r].max() < parts[n])
+    if movable is not None:
+        assert len(movable) == n
+        mov = [np.ascontiguousarray(m, dtype=np.uint8) for m in movable]
+        assert all(len(mov[r]) == sizes[r] for r in range(n))
     trace = np.zeros(max_trace, dtype=TRACE_DTYPE)
     iters = ctypes.c_int(0)
     const = ctypes.c_double(0)
-    mod = L.mvo_louvain(n, parts.ctypes.data, ctypes.cast(rp_ptrs, ctypes.c_void_p),
-                        ctypes.cast(ed_ptrs, ctypes.c_void_p), lower, thresh, ctypes.byref(iters),
-                        ctypes.cast(cm_ptrs, ctypes.c_void_p), trace.ctypes.data, max_trace, ctypes.byref(const))
+    converged = ctypes.c_int(1)
+    mod = L.mvo_louvain(n, parts.ctypes.data, arr(rps), arr(eds), lower, thresh, ctypes.byref(iters), arr(comm),
+                        trace.ctypes.data, max_trace, ctypes.byref(const), None if init is None else arr(init),
+                        int(stop_after), ctypes.byref(converged), None if mov is None else arr(mov), int(frontier),
+                        arr(mov_out))
     h = 0
     for r in range(n):
         h = (h + comm_hash(int(parts[r]), comm[r])) & 0xFFFFFFFFFFFFFFFF
     return {"modularity": mod, "iters": iters.value, "trace": trace[:min(iters.value, max_trace)].copy(),
-            "comm": comm, "constant": const.value, "chash_final": h}
+            "comm": comm, "constant": const.value, "chash_final": h, "converged": bool(converged.value),
+            "movable": mov_out}
 
 
 def have_reference():

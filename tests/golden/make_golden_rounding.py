@@ -5,7 +5,7 @@ of one fp64 counter sum (0.1 + 0.2 + 0.3 = 0.6000000000000001 in edge order, 0.6
 
 R1 cases start from singletons, so the reference itself records them: r1_ck1, r1_ck2 and r1_subrange on 1 rank, and
 r1_ck1 split over 2 ranks (A and B are ghosts of v's rank).  The R2 witness needs a warm start, which the reference's
-command line does not offer; its tests compare with tests/warm_oracle.c instead, which is pinned to the reference.
+command line does not offer; its tests compare with the C oracle's warm start instead, which is pinned to the reference.
 Before writing, this script asserts for every case: the reference's first iteration is the same on 1, 2 and 4 ranks,
 and the same graph with v's adjacency reversed gives a different first-iteration hash in the reference.
 Run where the reference binary can be built (python oracle/build_ref.py); the output is byte-identical on every run."""

@@ -68,6 +68,26 @@ def weighted_exact_cases():
         return json.load(f)["cases"]
 
 
+def golden_cases():
+    """name -> case of every reference trace in ref_traces.json, rmat_traces.json and (prefixed "dyadic_")
+    weighted_exact_traces.json."""
+    import json
+    import os
+    out = {}
+    for fn in ("ref_traces.json", "rmat_traces.json"):
+        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", fn)) as f:
+            out.update(json.load(f)["cases"])
+    for name, c in weighted_exact_cases().items():
+        out["dyadic_" + name] = c
+    return out
+
+
+def exact_cases():
+    """golden_cases() whose Comm sums are exact: unit weights (hand graphs: unit or k/4 weights), or dyadic weights."""
+    return {name: c for name, c in golden_cases().items()
+            if not ("-w" in c.get("args", []) or c.get("unit_weight") is False)}
+
+
 def dyadic_graph(case):
     """Global CSR (nv, rowptr, edges) of a dyadic-weight recipe from tests/golden/weighted_exact_traces.json."""
     kind = case["kind"]

@@ -5,7 +5,7 @@ Two modes, both in caller numbering on the whole graph (the shards only give the
 
 fp64 mode (`step`) restates the reference's arithmetic with its roundings.  k_i and every counter sum are summed
 sequentially in edge order; the self-loop weight is truncated through `long long`; the community degree a_c is summed
-in global vertex order from 0.0, as tests/warm_oracle.c does on a warm start (on the singletons of a cold start it is
+in global vertex order from 0.0, as the C oracle does on a warm start (on the singletons of a cold start it is
 k_c itself); the gain is `2.0*(eiy-eix) - ((2.0*k)*(ay-ax))*c` in that order; a candidate wins on a gain strictly
 above the best so far, starting from 0, and an equal non-zero gain goes to the smaller id (dspl.hpp:214-219); then
 the singleton veto (dspl.hpp:224-225).  All sums are sequential by construction (`seq_sum`: vectorised across groups,
@@ -108,7 +108,7 @@ def _pairs(G, X, edge_order=None):
 def _comm(G, X, vertex_order=None):
     size = np.bincount(X, minlength=G.nv)
     o = np.arange(G.nv) if vertex_order is None else np.asarray(vertex_order)
-    a = seq_sum(X[o], G.k[o], G.nv)                        # global vertex order, from 0.0 (tests/warm_oracle.c)
+    a = seq_sum(X[o], G.k[o], G.nv)                        # global vertex order, from 0.0 (the C oracle's init_comm)
     return size, a
 
 

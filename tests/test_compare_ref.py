@@ -14,7 +14,7 @@ import pytest
 from helpers import case_graph
 import compare_ref as CR
 import split_ref as SR
-import warm_oracle as W
+from oracle import oracle as O
 from test_quality_ref import CASES
 
 
@@ -128,7 +128,7 @@ def test_hand_values():
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_result_against_its_split(name):
     parts, rps, eds, _keep = case_graph(CASES[name])
-    X = np.concatenate(W.louvain(parts, rps, eds)["comm"])
+    X = np.concatenate(O.louvain(parts, rps, eds)["comm"])
     s = SR.split(parts, rps, eds, X)
     r = CR.compare(X, s["Y"])
     assert r["pairs_xy"] == r["pairs_y"] and r["cells"] == r["communities_y"] == s["components"], name

@@ -1,6 +1,6 @@
 """GPU tests of the movable set (mvgpu_set_movable, option "frontier", DESIGN.md §3.14).
 
-Every masked run is held bit for bit to the movable-set oracle (tests/movable_oracle.c): iteration count, every trace
+Every masked run is held bit for bit to the C oracle with the same set (oracle/louvain_oracle.c): iteration count, every trace
 record, the modularity, the final assignment and the returned set.  Covered: every unit and dyadic golden case on its
 own rank count (ranks > 1 share device 0 through the host transport) with random sets of density 0.01, 0.1 and 0.5,
 frontier 0 and 1, from singletons and warm; scan variants 3-6, renumbering 0/1/2, forced k_scan_heavy and every upload
@@ -15,8 +15,8 @@ import numpy as np
 import pytest
 
 from helpers import case_graph, dyadic_rgg, split_global
-import movable_oracle as MO
 import update_ref as U
+from oracle import oracle as O
 from test_gpu_parity import gpu  # noqa: F401  (fixture)
 from test_gpu_warm_start import EXE, Ranks, as_trace, cli
 from test_movable_oracle import CASES
@@ -46,7 +46,7 @@ def run(R, lower=-1.0):
 
 
 def oracle(parts, rps, eds, mask, frontier, init=None, **kw):
-    o = MO.louvain(parts, rps, eds, movable=None if mask is None else slices(parts, mask), frontier=frontier,
+    o = O.louvain(parts, rps, eds, movable=None if mask is None else slices(parts, mask), frontier=frontier,
                    init_comm=None if init is None else slices(parts, init), **kw)
     return {"mod": o["modularity"], "iters": o["iters"], "trace": as_trace(o["trace"]), "comm": np.concatenate(o["comm"]),
             "movable": np.concatenate(o["movable"]), "converged": o["converged"]}

@@ -1,7 +1,7 @@
 """Shard updates on the device (mvgpu_update_shard, LouvainGPU.update_shard; DESIGN.md §3.11), against the NumPy
 restatement tests/update_ref.py element for element, against the device generator (`-p 0` + extras == `-p 5`), and
 through the Louvain phase: a cold run on an updated shard equals a cold run on the same graph uploaded fresh, and a warm
-run from the pre-update result equals the warm-start oracle started from that assignment."""
+run from the pre-update result equals the C oracle started from that assignment."""
 import json
 import os
 
@@ -223,7 +223,7 @@ def louvain_graphs():
 @pytest.mark.parametrize("world", [1, 2, 4])
 def test_louvain_after_update(gpu, world):
     """Cold run on the updated shard == cold run on the updated graph uploaded fresh (bit for bit); warm run from the
-    pre-update result == the warm-start oracle from that assignment; communities() keeps the pre-update result and the
+    pre-update result == the C oracle started from that assignment; communities() keeps the pre-update result and the
     initial assignment survives the update."""
     for name, nv, before, dele, ins in louvain_graphs():
         after = U.apply(0, before[0], before[1], dele, ins)
@@ -252,7 +252,7 @@ def test_louvain_after_update(gpu, world):
 def test_dynamic_graph_warm_start_through_update(gpu):
     """test_gpu_warm_start.py::test_dynamic_graph_warm_start's scenario (-p 0 result, then -p 5) without re-uploading:
     run, update, communities(), set_initial_communities, run."""
-    import warm_oracle as W
+    from oracle import oracle as O
     from minivite_b200 import gpu as G
     from minivite_b200 import hostgraph as hg
     ss0 = hg.generate_rgg(65536, 1)
@@ -268,7 +268,7 @@ def test_dynamic_graph_warm_start_through_update(gpu):
         prev = g.communities().copy()
         g.set_initial_communities(prev)
         mod, iters = g.louvain()
-        ref = W.louvain(s5.parts, [s5.rowptr], [s5.edges], init_comm=[prev])
+        ref = O.louvain(s5.parts, [s5.rowptr], [s5.edges], init_comm=[prev])
         assert (iters, mod) == (ref["iters"], ref["modularity"])
         assert as_trace(g.trace()) == as_trace(ref["trace"])
         assert np.array_equal(g.communities(), ref["comm"][0])

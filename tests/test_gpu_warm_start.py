@@ -4,8 +4,8 @@ A run stopped after its accepted iteration k and resumed from its assignment wit
 continue the reference's run exactly (DESIGN.md §3.9; tests/test_oracle_warm_start.py checks that argument on the C
 oracle).  So every unit and dyadic golden trace doubles as a split-and-resume test: the stopped run must give the
 golden prefix and the oracle's checkpoint assignment C_k array for array, the resumed run the golden suffix, iteration
-count, modularity and final hash bit for bit.  Arbitrary starting assignments are checked against the oracle's
-warm-start variant (tests/warm_oracle.py) started from the same assignment, on 1 rank and on 2 and 4 ranks sharing device 0 (host transport)."""
+count, modularity and final hash bit for bit.  Arbitrary starting assignments are checked against the C oracle
+started from the same assignment, on 1 rank and on 2 and 4 ranks sharing device 0 (host transport)."""
 import json
 import os
 import re
@@ -16,8 +16,7 @@ import threading
 import numpy as np
 import pytest
 
-from helpers import case_graph, random_graph, split_global, weighted_exact_cases
-import warm_oracle as W
+from helpers import case_graph, exact_cases, random_graph, split_global
 from oracle import oracle as O
 from test_gpu_parity import gpu  # noqa: F401  (fixture)
 
@@ -25,21 +24,6 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 EXE = os.path.join(ROOT, "bin", "miniVite_b200")
-
-
-def exact_cases():
-    """name -> case for every golden case whose Comm sums are exact: unit weights or dyadic weights."""
-    out = {}
-    for fn in ("ref_traces.json", "rmat_traces.json"):
-        with open(os.path.join(GOLDEN, fn)) as f:
-            for name, c in json.load(f)["cases"].items():
-                if not ("-w" in c.get("args", []) or c.get("unit_weight") is False):
-                    out[name] = c
-    for name, c in weighted_exact_cases().items():
-        out["dyadic_" + name] = c
-    return out
-
-
 CASES = exact_cases()
 
 
@@ -129,7 +113,7 @@ class Ranks:
 
 def oracle_run(parts, rps, eds, init=None, **kw):
     init_slices = None if init is None else [init[parts[r]:parts[r + 1]] for r in range(len(rps))]
-    res = W.louvain(parts, rps, eds, init_comm=init_slices, **kw)
+    res = O.louvain(parts, rps, eds, init_comm=init_slices, **kw)
     return {"mod": res["modularity"], "iters": res["iters"], "trace": as_trace(res["trace"]),
             "comm": np.concatenate(res["comm"]), "converged": res["converged"]}
 
@@ -306,7 +290,7 @@ def test_dynamic_graph_warm_start(gpu, unit):
         mod, iters = g.louvain()
         comm = g.communities().copy()
         tr = as_trace(g.trace())
-        ref = W.louvain(s5.parts, [s5.rowptr], [s5.edges], init_comm=[prev])
+        ref = O.louvain(s5.parts, [s5.rowptr], [s5.edges], init_comm=[prev])
         if unit:
             assert (iters, mod) == (ref["iters"], ref["modularity"])
             assert tr == as_trace(ref["trace"])

@@ -243,7 +243,7 @@ WITNESS_OPTS = [dict(scan_variant=sv, reorder=ro, **({"region_size": 32} if ro e
 @pytest.mark.parametrize("world", [1, 2, 4])
 def test_rounding_witnesses_bit_exact(gpu, world):
     """The witness step is bit-exact in its targets, moved count and hash: against the reference's first iteration
-    (tests/golden/rounding_traces.json) and the C oracle's X1 for R1, against tests/warm_oracle.c's T(X) for R2."""
+    (tests/golden/rounding_traces.json) and the C oracle's X1 for R1, against the C oracle's warm T(X) for R2."""
     for name in ("r1_ck1", "r1_ck2", "r1_subrange", "r2_own"):
         parts, rps, eds, X, T_or, tr_or, _c = witness_step(name, world)
         gold = [c for c in WITNESS_GOLDEN.values() if c["witness"] == name]

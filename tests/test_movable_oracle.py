@@ -1,34 +1,13 @@
-"""CPU tests of the movable-set oracle (tests/movable_oracle.c, DESIGN.md §3.14) before any GPU run: with everything
-movable it is the warm-start oracle; a frozen vertex keeps its community in one step exactly as tests/step_ref.py's step
+"""CPU tests of the C oracle's movable set (movable, frontier; DESIGN.md §3.14) before any GPU run: with everything
+movable it is the run without a set; a frozen vertex keeps its community in one step exactly as tests/step_ref.py's step
 with that target overwritten; the frontier grows like a plain per-record loop; stop and resume with the returned set
 continues the run exactly; and the result does not depend on the shard count."""
-import json
-import os
-
 import numpy as np
 import pytest
 
-from helpers import case_graph, global_csr, split_global, weighted_exact_cases
-import movable_oracle as MO
+from helpers import case_graph, exact_cases, global_csr, split_global
 import step_ref as S
-import warm_oracle as W
 from oracle import oracle as O
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def exact_cases():
-    """name -> case for every golden case whose Comm sums are exact: unit weights, or dyadic weights."""
-    out = {}
-    for fn in ("ref_traces.json", "rmat_traces.json"):
-        with open(os.path.join(GOLDEN, fn)) as f:
-            for name, c in json.load(f)["cases"].items():
-                if not ("-w" in c.get("args", []) or c.get("unit_weight") is False):
-                    out[name] = c
-    for name, c in weighted_exact_cases().items():
-        out["dyadic_" + name] = c
-    return out
-
 
 CASES = exact_cases()
 # graphs that do not depend on the rank count, so that 1, 2 and 4 shards of one graph can be compared
@@ -54,21 +33,24 @@ def same_run(a, b):
 
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_all_movable_is_the_warm_oracle(name):
+    """An all-ones set, with frontier 0 and 1, is the run without a set (which reports an all-ones set); so is frontier 1
+    without a set."""
     parts, rps, eds, _keep = case_graph(CASES[name])
-    ref = W.louvain(parts, rps, eds)
+    ref = O.louvain(parts, rps, eds)
+    assert all(np.all(m == 1) for m in ref["movable"])
     ones = [np.ones(int(parts[r + 1] - parts[r]), np.uint8) for r in range(len(rps))]
     for frontier in (0, 1):
-        res = MO.louvain(parts, rps, eds, movable=ones, frontier=frontier)
+        res = O.louvain(parts, rps, eds, movable=ones, frontier=frontier)
         same_run(res, ref)
         assert all(np.all(m == 1) for m in res["movable"])
-    same_run(MO.louvain(parts, rps, eds), ref)
+    same_run(O.louvain(parts, rps, eds, frontier=1), ref)
 
 
 @pytest.mark.parametrize("name", ["rgg_n16384_p1", "hand_loops_multi_p2", "rmat_s14_p2_b"])
 def test_all_frozen_moves_nothing(name):
     parts, rps, eds, _keep = case_graph(CASES[name])
     zeros = [np.zeros(int(parts[r + 1] - parts[r]), np.uint8) for r in range(len(rps))]
-    res = MO.louvain(parts, rps, eds, movable=zeros, frontier=0)
+    res = O.louvain(parts, rps, eds, movable=zeros, frontier=0)
     # iteration 1 moves nothing and is accepted against lower = -1; iteration 2 repeats it and fails the exit test
     assert res["iters"] == 2 and res["converged"] and [int(t["moved"]) for t in res["trace"]] == [0, 0]
     assert res["trace"][0]["modularity"] == res["trace"][1]["modularity"]
@@ -84,7 +66,7 @@ def test_one_masked_step_is_step_ref_with_frozen_targets(name, density):
     mask = random_masks(parts, density, 7)
     for X0 in (None, np.random.default_rng(3).integers(0, G.nv, G.nv)):
         init = None if X0 is None else [X0[parts[r]:parts[r + 1]] for r in range(len(rps))]
-        res = MO.louvain(parts, rps, eds, movable=mask, init_comm=init, max_trace=1, thresh=-1.0, stop_after=1)
+        res = O.louvain(parts, rps, eds, movable=mask, init_comm=init, max_trace=1, thresh=-1.0, stop_after=1)
         X = np.arange(G.nv) if X0 is None else X0
         T = S.step(G, X, res["constant"])["target"]
         frozen = np.concatenate(mask) == 0
@@ -116,7 +98,7 @@ def test_frontier_growth_is_a_per_record_loop(name):
     mask = random_masks(parts, 0.05, 11)
     X = np.arange(int(parts[-1]))
     for k in (1, 2, 3):
-        a = MO.louvain(parts, rps, eds, movable=mask, frontier=1, init_comm=[X[parts[r]:parts[r + 1]] for r in range(len(rps))],
+        a = O.louvain(parts, rps, eds, movable=mask, frontier=1, init_comm=[X[parts[r]:parts[r + 1]] for r in range(len(rps))],
                        stop_after=1)
         if a["converged"]:
             break
@@ -129,12 +111,12 @@ def test_frontier_growth_is_a_per_record_loop(name):
 def test_stop_and_resume_with_the_returned_set(name):
     parts, rps, eds, _keep = case_graph(CASES[name])
     mask = random_masks(parts, 0.1, 5)
-    full = MO.louvain(parts, rps, eds, movable=mask, frontier=1)
+    full = O.louvain(parts, rps, eds, movable=mask, frontier=1)
     iters = full["iters"]
     for k in sorted({k for k in (1, iters // 2, iters - 1) if 1 <= k <= iters - 1}):
-        a = MO.louvain(parts, rps, eds, movable=mask, frontier=1, stop_after=k)
+        a = O.louvain(parts, rps, eds, movable=mask, frontier=1, stop_after=k)
         assert not a["converged"] and run_trace(a) == run_trace(full)[:k], (name, k)
-        b = MO.louvain(parts, rps, eds, movable=a["movable"], frontier=1, init_comm=a["comm"], lower=a["modularity"])
+        b = O.louvain(parts, rps, eds, movable=a["movable"], frontier=1, init_comm=a["comm"], lower=a["modularity"])
         assert k + b["iters"] == iters and run_trace(b) == run_trace(full)[k:], (name, k)
         assert repr(b["modularity"]) == repr(full["modularity"]) and b["chash_final"] == full["chash_final"], (name, k)
         for x, y in zip(b["movable"], full["movable"]):
@@ -149,7 +131,7 @@ def test_same_result_on_1_2_and_4_shards(name, frontier):
     runs = []
     for p in (1, 2, 4):
         parts, rps, eds = split_global(nv, rowptr, edges, p)
-        res = MO.louvain(parts, rps, eds, movable=[mask[parts[r]:parts[r + 1]] for r in range(p)], frontier=frontier)
+        res = O.louvain(parts, rps, eds, movable=[mask[parts[r]:parts[r + 1]] for r in range(p)], frontier=frontier)
         runs.append((res["iters"], repr(res["modularity"]), run_trace(res), np.concatenate(res["comm"]).tolist(),
                      np.concatenate(res["movable"]).tolist()))
     assert runs[0] == runs[1] == runs[2]

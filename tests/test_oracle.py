@@ -5,7 +5,7 @@ import os
 import numpy as np
 import pytest
 
-from helpers import assert_dyadic_exact, assert_trace_matches, case_graph, global_csr, weighted_exact_cases
+from helpers import assert_dyadic_exact, assert_trace_matches, case_graph, global_csr, golden_cases, weighted_exact_cases
 from oracle import oracle as O
 
 
@@ -44,6 +44,26 @@ def test_oracle_matches_every_golden_case(golden):
         comm = np.concatenate(res["comm"])
         assert_trace_matches(case, res["iters"], res["modularity"], res["trace"], res["chash_final"], comm)
         assert repr(res["constant"]) == case["constant"], name
+
+
+GOLDEN_CASES = golden_cases()
+
+
+@pytest.mark.parametrize("name", sorted(GOLDEN_CASES))
+def test_neutral_extensions_are_the_pinned_run(name):
+    """init_comm set to the identity, movable set to all ones, and stop_after=0 each give the plain call's run bit for
+    bit: trace, modularity, 1/(2m), final hash and assignment."""
+    parts, rps, eds, _keep = case_graph(GOLDEN_CASES[name])
+    ref = O.louvain(parts, rps, eds)
+    ident = [np.arange(parts[r], parts[r + 1], dtype=np.int64) for r in range(len(rps))]
+    ones = [np.ones(int(parts[r + 1] - parts[r]), np.uint8) for r in range(len(rps))]
+    for kw in (dict(init_comm=ident), dict(movable=ones), dict(stop_after=0)):
+        res = O.louvain(parts, rps, eds, **kw)
+        assert (res["iters"], repr(res["modularity"]), repr(res["constant"]), res["chash_final"], res["converged"]) == \
+            (ref["iters"], repr(ref["modularity"]), repr(ref["constant"]), ref["chash_final"], True), (name, kw.keys())
+        assert res["trace"].tobytes() == ref["trace"].tobytes(), (name, kw.keys())
+        for x, y in zip(res["comm"], ref["comm"]):
+            assert np.array_equal(x, y), (name, kw.keys())
 
 
 def test_partition_invariance_unit_weights(golden):

@@ -4,33 +4,14 @@ The modularity the reference reports for iteration k is mixed: e_in is measured 
 and a2 on the one it wrote (X_k).  So for every accepted iteration k of a golden trace
     T[k].modularity == fabs(e_in(X_{k-1})*c - (a2(X_k)*c)*c)   bit for bit
 when the sums are exact (unit and dyadic weights).  X_0 is the singleton assignment and X_k comes from the C oracle's
-stop points (tests/warm_oracle.py).  That pins the restatement -- and through it the device evaluation -- to the
+stop points (stop_after).  That pins the restatement -- and through it the device evaluation -- to the
 reference's own goldens."""
-import json
-import os
-
 import numpy as np
 import pytest
 
-from helpers import case_graph, random_graph, split_global, weighted_exact_cases
+from helpers import case_graph, exact_cases, random_graph, split_global
 import quality_ref as QR
-import warm_oracle as W
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def exact_cases():
-    """name -> case for every golden case whose sums are exact: unit weights, or dyadic weights."""
-    out = {}
-    for fn in ("ref_traces.json", "rmat_traces.json"):
-        with open(os.path.join(GOLDEN, fn)) as f:
-            for name, c in json.load(f)["cases"].items():
-                if not ("-w" in c.get("args", []) or c.get("unit_weight") is False):
-                    out[name] = c
-    for name, c in weighted_exact_cases().items():
-        out["dyadic_" + name] = c
-    return out
-
+from oracle import oracle as O
 
 CASES = exact_cases()
 
@@ -50,7 +31,7 @@ def identity_points(case):
 def assignment_after(parts, rps, eds, k):
     if k == 0:
         return np.arange(int(parts[-1]), dtype=np.int64)
-    res = W.louvain(parts, rps, eds, stop_after=k)
+    res = O.louvain(parts, rps, eds, stop_after=k)
     assert res["iters"] == k and not res["converged"]
     return np.concatenate(res["comm"])
 

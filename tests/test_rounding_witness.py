@@ -9,7 +9,6 @@ import numpy as np
 import pytest
 
 import step_ref as S
-import warm_oracle as W
 from helpers import (WITNESS_A, WITNESS_B, WITNESS_U, WITNESS_V, assert_trace_matches, reversed_adjacency,
                      rounding_witness, split_global)
 from oracle import oracle as O
@@ -24,7 +23,7 @@ def witness_step(name, p=1, reverse=False):
         edges = reversed_adjacency(rowptr, edges, WITNESS_V)
     parts, rps, eds = split_global(nv, rowptr, edges, p)
     X = np.arange(nv, dtype=np.int64) if X is None else X
-    res = W.louvain(parts, rps, eds, init_comm=[X[parts[r]:parts[r + 1]] for r in range(p)], stop_after=1)
+    res = O.louvain(parts, rps, eds, init_comm=[X[parts[r]:parts[r + 1]] for r in range(p)], stop_after=1)
     return parts, rps, eds, X, np.concatenate(res["comm"]), res["trace"][0], res["constant"]
 
 

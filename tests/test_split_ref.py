@@ -9,7 +9,7 @@ import pytest
 from helpers import case_graph, split_global
 import quality_ref as QR
 import split_ref as SR
-import warm_oracle as W
+from oracle import oracle as O
 from test_quality_ref import CASES, hand_assignments, hand_graphs
 
 EDGE = np.dtype([("tail", "<i8"), ("weight", "<f8")])
@@ -121,7 +121,7 @@ def test_hand_case_values():
 def test_split_of_oracle_results(name):
     case = CASES[name]
     parts, rps, eds, _keep = case_graph(case)
-    X = np.concatenate(W.louvain(parts, rps, eds)["comm"])
+    X = np.concatenate(O.louvain(parts, rps, eds)["comm"])
     s = SR.split(parts, rps, eds, X)
     Y = s["Y"]
     qx, qy = QR.quality(parts, rps, eds, X), QR.quality(parts, rps, eds, Y)
@@ -139,6 +139,6 @@ def test_rmat_fixture_counts():
     want = {"rmat_s14_p1": (8251, 10500, 759), "rmat_s17_p1": (70303, 86659, 4282)}
     for name, counts in want.items():
         parts, rps, eds, _keep = case_graph(CASES[name])
-        X = np.concatenate(W.louvain(parts, rps, eds)["comm"])
+        X = np.concatenate(O.louvain(parts, rps, eds)["comm"])
         s = SR.split(parts, rps, eds, X)
         assert (s["communities"], s["components"], s["disconnected"]) == counts, name

@@ -2,7 +2,7 @@
 taken in other orders.
 
 fp64 mode must give the oracle's first-iteration targets, moved count and hash from singletons on golden cases of every
-kind (unit, dyadic and the three Euclidean ones, whose sums round), and tests/warm_oracle.c's single step from its own
+kind (unit, dyadic and the three Euclidean ones, whose sums round), and the C oracle's single warm step from its own
 checkpoints and from random assignments.  Certified mode must contain every gain that other summation orders give: the
 community degrees in reverse and random vertex order, and the heavy vertices' counters in permuted edge order."""
 import json
@@ -12,7 +12,6 @@ import numpy as np
 import pytest
 
 import step_ref as S
-import warm_oracle as W
 from helpers import case_graph, random_graph, split_global, weighted_exact_cases
 from oracle import oracle as O
 
@@ -43,8 +42,8 @@ def chash(parts, T):
 
 
 def one_step(parts, rps, eds, X):
-    """warm_oracle's single accepted step from X: (T(X), trace[0], constant)."""
-    res = W.louvain(parts, rps, eds, init_comm=[X[parts[r]:parts[r + 1]] for r in range(len(rps))], stop_after=1)
+    """The C oracle's single accepted step from X: (T(X), trace[0], constant)."""
+    res = O.louvain(parts, rps, eds, init_comm=[X[parts[r]:parts[r + 1]] for r in range(len(rps))], stop_after=1)
     return np.concatenate(res["comm"]), res["trace"][0], res["constant"]
 
 
@@ -116,7 +115,7 @@ def random_assignments(nv, seed):
 def warm_inputs(parts, rps, eds, iters):
     out = {}
     for k in sorted({k for k in (1, iters // 2, iters - 1) if k >= 1}):
-        out[f"ck{k}"] = np.concatenate(W.louvain(parts, rps, eds, stop_after=k)["comm"])
+        out[f"ck{k}"] = np.concatenate(O.louvain(parts, rps, eds, stop_after=k)["comm"])
     out.update(random_assignments(int(parts[-1]), 3))
     return out
 
@@ -140,7 +139,7 @@ def test_warm_step_matches_warm_oracle(name):
 def test_warm_step_matches_warm_oracle_general_graphs():
     for gname, (parts, rps, eds) in general_graphs().items():
         G = S.Graph(parts, rps, eds)
-        res = W.louvain(parts, rps, eds)
+        res = O.louvain(parts, rps, eds)
         for xname, X in warm_inputs(parts, rps, eds, res["iters"]).items():
             T_or, tr, const = one_step(parts, rps, eds, X)
             r = S.step(G, X, const)
@@ -205,7 +204,7 @@ def test_certificate_contains_other_orders(heavy_deg):
     rng = np.random.default_rng(11)
     for gname, (parts, rps, eds) in general_graphs().items():
         G = S.Graph(parts, rps, eds)
-        res = W.louvain(parts, rps, eds)
+        res = O.louvain(parts, rps, eds)
         const = res["constant"]
         inputs = {"X0": np.arange(G.nv, dtype=np.int64)}
         inputs.update(warm_inputs(parts, rps, eds, res["iters"]))
