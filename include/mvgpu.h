@@ -234,6 +234,9 @@ int mvgpu_get_communities_device(mvgpu_ctx *ctx, const int32_t **d_out);
 /* Options: "trace" (0/1: record moved/chash per iteration, default 0), "max_iters" (safety cap,
  * default 10000), "force_weighted" (0/1: use the fp64 path even for unit weights, default 0),
  * "force_heavy_deg" (test hook: treat vertices with degree > value as high-degree, default 0 = off),
+ * "scan_ctas" (test hook: k > 0 caps the grids of the persistent scan kernels k_scan_pw and k_scan_pq at k CTAs, so
+ * every warp strides over many 32-vertex groups even on a small shard, as a large shard or a part with fewer SMs does;
+ * default 0 = resident CTAs per SM x SMs; negative values are refused; identical results),
  * "scan_variant" (6 (default): iterations 2 and 4 run k_scan_pw, iteration 3 k_scan_pq, and from iteration 5 on
  * k_scan_pq runs if it beat the geometric mean of its neighbours, else k_scan_pw; 5 = k_scan_pq: persistent warps fed by TMA bulk copies, boundary vertices reduced from a
  * per-warp ring -- unit weights; iteration 1 and weighted graphs run k_scan_pw; 4 = k_scan_pw throughout; 3 =

@@ -228,6 +228,7 @@ struct mvgpu_ctx {
   int opt_trace = 0, opt_force_weighted = 0, opt_scan_variant = 6, opt_cache_policy = 5, opt_reorder = 2, opt_region = 512, opt_comm_mode = 1, opt_compact_upload = 0, opt_host_threads = 8, opt_first_iter = 1, opt_host_transport = 0, opt_frontier = 0;
   long long opt_upload_chunk = 4LL << 20;
   long long opt_max_iters = 10000, opt_force_heavy_deg = 0, opt_stop_after = 0;
+  int opt_scan_ctas = 0;               // test hook: > 0 caps the persistent scan grids at that many CTAs (0 = occupancy x SMs)
   // warm start (mvgpu_set_initial_communities): caller-numbered community ids of this shard, until the next graph
   DevBuf<int32_t> init_comm;
   bool have_init = false;
@@ -535,7 +536,7 @@ int launch_scan_t(mvgpu_ctx *c, const ScanParams &sp, bool first, const uint8_t 
       if (pq_ctas_per_sm < 1) return fail("k_scan_pq cannot be made resident");
     }
     const int ngroups = (int)((c->lnv + 31) / 32);
-    const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, pq_ctas_per_sm * c->num_sms);
+    const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, c->opt_scan_ctas > 0 ? c->opt_scan_ctas : pq_ctas_per_sm * c->num_sms);
     k_scan_pq<MULTI, TRACE, MASKED><<<grid, kPwWarps * 32, pq_smem_bytes(), c->stream>>>(sp, ngroups, mov);
     c->tm.kernel_launches++; c->tm.scan_launches++;
   } else if (tiles > 0 && c->opt_scan_variant >= 4) {
@@ -548,7 +549,7 @@ int launch_scan_t(mvgpu_ctx *c, const ScanParams &sp, bool first, const uint8_t 
       if (pw_ctas_per_sm < 1) return fail("k_scan_pw cannot be made resident");
     }
     const int ngroups = (int)((c->lnv + 31) / 32);
-    const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, pw_ctas_per_sm * c->num_sms);
+    const int grid = std::min((ngroups + kPwWarps - 1) / kPwWarps, c->opt_scan_ctas > 0 ? c->opt_scan_ctas : pw_ctas_per_sm * c->num_sms);
     if (UNIT && first) {
       k_scan_pw<UNIT, MULTI, TRACE, UNIT && !MASKED, MASKED><<<grid, kPwWarps * 32, pw_smem_bytes<UNIT>(), c->stream>>>(sp, ngroups, mov);
       c->lay.first_ran = true;
@@ -2514,6 +2515,7 @@ int mvgpu_set_option(mvgpu_ctx *c, const char *name, int64_t value) {
   else if (n == "max_iters") { if (value < 1) return fail("max_iters < 1"); c->opt_max_iters = value; }
   else if (n == "force_weighted") c->opt_force_weighted = value != 0;
   else if (n == "force_heavy_deg") c->opt_force_heavy_deg = value;
+  else if (n == "scan_ctas") { if (value < 0 || value > INT32_MAX) return fail("scan_ctas must be >= 0"); c->opt_scan_ctas = (int)value; }
   else if (n == "scan_variant") { if (value < 3 || value > 6) return fail("scan_variant must be 6 (measure and choose, default), 5 (k_scan_pq), 4 (k_scan_pw) or 3 (k_scan_ws)"); c->opt_scan_variant = (int)value; }
   else if (n == "cache_policy") c->opt_cache_policy = (int)value;
   else if (n == "reorder") c->opt_reorder = (int)value;
