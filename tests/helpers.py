@@ -68,6 +68,22 @@ def weighted_exact_cases():
         return json.load(f)["cases"]
 
 
+def rank_cases():
+    """name -> case of tests/golden/rank_traces.json: the unmodified reference on 3..16 ranks, including splits that
+    leave ranks with one vertex or none (tests/golden/make_golden_ranks.py)."""
+    import json
+    import os
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "rank_traces.json")) as f:
+        return json.load(f)["cases"]
+
+
+def one_shard(parts, rowptrs, edge_lists):
+    """The same graph as one shard: (parts, [rowptr], [edges])."""
+    offs = np.cumsum([0] + [int(r[-1]) for r in rowptrs[:-1]])
+    rowptr = np.concatenate([[0]] + [np.asarray(r[1:], np.int64) + o for r, o in zip(rowptrs, offs)]).astype(np.int64)
+    return np.array([0, int(parts[-1])], np.int64), [rowptr], [np.concatenate(edge_lists)]
+
+
 def golden_cases():
     """name -> case of every reference trace in ref_traces.json, rmat_traces.json and (prefixed "dyadic_")
     weighted_exact_traces.json."""

@@ -43,11 +43,21 @@ def _worker(rank, world, port, case_name, out_dir, opts):
         from test_gpu_layout import keep_order_graph
         nv, parts, rowptr, edges = keep_order_graph(world)
         _, rps, eds = split_global(nv, rowptr, edges, world)
+    elif case_name.startswith("empty_first:"):  # every rank but the last owns no vertex (tests/test_gpu_rank_counts.py)
+        from helpers import global_csr, rank_cases, split_global
+        nv, rowptr, edges = global_csr(rank_cases()[case_name[len("empty_first:"):]])
+        parts, rps, eds = split_global(nv, rowptr, edges, 1)
+        parts = np.array([0] * world + [nv], np.int64)
+        rps, eds = [np.zeros(1, np.int64)] * (world - 1) + rps, [eds[0][:0]] * (world - 1) + eds
     else:
         if case_name.startswith("wexact:"):      # a dyadic-weight case of weighted_exact_traces.json
             from helpers import weighted_exact_cases
             case_name = case_name[len("wexact:"):]
             golden = weighted_exact_cases()
+        elif case_name.startswith("ranks:"):     # a case of rank_traces.json (3..16 ranks, uneven splits)
+            from helpers import rank_cases
+            case_name = case_name[len("ranks:"):]
+            golden = rank_cases()
         else:
             golden = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_traces.json")))["cases"]
         case = dict(golden[case_name])
@@ -97,13 +107,22 @@ def check(res, case, exact=True):
                                              ("file_balanced_n16384_p2", 2), ("file_balanced_n16384_p4", 4),
                                              # SURVEY.md 8(c) known answers of `miniVite -n 524288` (auto renumbering on)
                                              ("file_rgg_n524288_s1_p1", 2), ("file_rgg_n524288_s8_p8", 2),
-                                             ("file_rgg_n524288_s8_p8", 8)])
+                                             ("file_rgg_n524288_s8_p8", 8),
+                                             # uneven rank counts (tests/golden/rank_traces.json)
+                                             ("ranks:file_rgg_n16384_s1_p3", 3), ("ranks:file_rgg_n32768_s8_p5", 5),
+                                             ("ranks:file_rgg_n16384_s1_p6", 6), ("ranks:hand_star41_p7", 7),
+                                             ("ranks:file_rgg_n32768_s8_p7", 7)])
 def test_multi_gpu_matches_reference_ranks(tmp_path, golden, case_name, world):
     if ngpus() < world:
         pytest.skip(f"needs {world} GPUs")
     res = run_ranks(tmp_path, world, case_name)
-    check(res, golden[case_name])
-    if world > 1 and golden[case_name]["kind"] not in ("hand",):
+    if case_name.startswith("ranks:"):
+        from helpers import rank_cases
+        case = rank_cases()[case_name[len("ranks:"):]]
+    else:
+        case = golden[case_name]
+    check(res, case)
+    if world > 1 and case["kind"] not in ("hand",):
         assert res["info"]["nghost"] > 0
 
 
@@ -158,6 +177,10 @@ def test_multi_gpu_nccl_collectives_mode(tmp_path, golden):
         check(res, golden[name])
         res = run_ranks(tmp_path, 2, name, comm_mode=0, reorder=1, region_size=64)
         check(res, golden[name])
+    # rank 0 owns no vertex: empty send and receive counts in every NCCL exchange
+    from helpers import rank_cases
+    res = run_ranks(tmp_path, 2, "empty_first:hand_clique_ring_p3", comm_mode=0)
+    check(res, rank_cases()["hand_clique_ring_p3"])
 
 
 def test_multi_gpu_weighted_and_heavy(tmp_path, golden):

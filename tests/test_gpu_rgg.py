@@ -14,7 +14,9 @@ pytestmark = pytest.mark.gpu
                                                 (1048576, 8, [0, 5], True, False),
                                                 # -l: the reference's LCG stream, a different point pattern per strip
                                                 (16384, 1, [0], True, True), (16384, 2, [0, 1], True, True),
-                                                (32768, 4, [0, 1, 2, 3], False, True), (1048576, 8, [0, 4, 7], True, True)])
+                                                (32768, 4, [0, 1, 2, 3], False, True), (1048576, 8, [0, 4, 7], True, True),
+                                                # 16 strips, plain and -l
+                                                (16384, 16, [0, 7, 15], True, False), (16384, 16, [0, 9, 15], True, True)])
 def test_device_generator_matches_host_generator(n, p, ranks, unit, lcg):
     from minivite_b200 import gpu as G
     from minivite_b200 import hostgraph as hg
@@ -100,7 +102,8 @@ def test_device_generator_random_edges(n, unit, lcg, pct):
 
 
 @pytest.mark.parametrize("n,p,unit,lcg,pct", [(16384, 2, True, False, 20.0), (32768, 4, False, False, 10.0),
-                                              (131072, 8, False, True, 5.0), (16384, 4, True, False, 0.004)])
+                                              (131072, 8, False, True, 5.0), (16384, 4, True, False, 0.004),
+                                              (16384, 16, True, False, 20.0)])
 def test_device_generator_random_edges_on_ranks(n, p, unit, lcg, pct):
     """-p on p ranks (threads sharing device 0, host transport): every rank replays all p draw streams and keeps the
     forward edges of its own stream plus the reverse edges the other streams send it; weighted far pairs take the
