@@ -73,6 +73,20 @@ int mvgpu_get_unique_id(void *id128);
 int mvgpu_comm_init(mvgpu_ctx *ctx, const void *id128);
 
 /* ---- graph hand-off -------------------------------------------------------------------------- */
+/* Shard replacement (mvgpu_upload_shard, mvgpu_upload_shard32, mvgpu_attach_shard_device, mvgpu_generate_rgg_shard[_ex]):
+ * every check runs before anything changes, so a refused call changes nothing -- the current shard, its initial
+ * assignment, movable set, last run, evaluation and comparison stay as they were (a generated shard is built in arrays
+ * of its own and takes the current one's place only at the end).  After success the context holds the new shard and
+ * nothing of the old one's: the initial assignment, the movable set, the NULL forms of evaluate / split / compare, the
+ * per-community getters and the per-vertex result getters (mvgpu_get_communities, mvgpu_get_communities32,
+ * mvgpu_get_communities_device) all wait for the new shard's first run or call, and mvgpu_get_shard_info reports 0 in
+ * info[2..5] until its first run.  A failure after the checks (a device allocation or copy) leaves the context with no
+ * shard: every compute entry point then refuses until the next successful upload / attach / generate.  With several
+ * ranks that refusal is local (it comes before the first collective), so the peers of a rank without a shard wait in
+ * their first collective: every rank must hold a shard before a collective call. 
+ * In a multi-rank run every rank must hold a shard of the same partition (nv_global and parts): mvgpu_louvain,
+ * mvgpu_evaluate_communities, mvgpu_split_communities and mvgpu_compare_communities compare the ranks' partitions in
+ * their first all-reduce and fail on every rank with "ranks disagree on the partition" otherwise. */
 /* Host arrays of a reference Graph shard (graph.hpp:289-293): copies them to HBM.
  * parts: nranks+1 global vertex offsets (graph.hpp:109-113 or the -b bins, graph.hpp:511);
  * edge_indices: lnv+1 LOCAL offsets; edge_list: lne records {int64 tail; double weight}. */
@@ -117,7 +131,7 @@ int mvgpu_update_shard(mvgpu_ctx *ctx, int64_t n_del, const int64_t *del_src, co
  * (dspl.hpp:1430); *modularity is prevMod (dspl.hpp:1440).  Collective over all ranks. */
 int mvgpu_louvain(mvgpu_ctx *ctx, double lower, double thresh, int *iters, double *modularity);
 
-/* Warm start: the next runs on this shard start from `comm` (lnv global community ids in the caller's vertex numbering,
+/* Warm start (a refused call changes nothing): the next runs on this shard start from `comm` (lnv global community ids in the caller's vertex numbering,
  * the form mvgpu_get_communities returns) instead of singletons.  Every id must lie in [0, nv); id c names the vertex
  * whose owner keeps the community's Comm record, as in the reference -- the community need not contain vertex c, need
  * not be contiguous and may be owned by another rank.  The array is copied and validated at call time (errors are
@@ -137,7 +151,7 @@ int mvgpu_get_converged(mvgpu_ctx *ctx, int *converged);
  * (default) M_k = M in every iteration; 1: M_{k+1} = M_k + { u : a vertex v != u with a stored record v->u has target !=
  * current in iteration k } (own and ghost tails; u may be owned by another rank); a rejected last iteration does not grow
  * it.  An all-ones set gives the same bits as no set.
- * mvgpu_set_movable copies the array at call time (errors are local); it stays in effect for every later mvgpu_louvain on
+ * mvgpu_set_movable copies the array at call time (errors are local; a refused call changes nothing); it stays in effect for every later mvgpu_louvain on
  * this shard until NULL clears it (= everything movable) or the next upload / attach / generate; mvgpu_update_shard keeps
  * it.  In a multi-rank run every rank or none must set one (checked at the start of mvgpu_louvain, which then fails on
  * every rank).  Not for mvgpu_louvain32. */
@@ -226,9 +240,11 @@ int mvgpu_compare_communities(mvgpu_ctx *ctx, const int64_t *x, const int64_t *y
  * failed one, and after the next upload, attach or generate.  Any of the four arrays may be NULL (not written). */
 int mvgpu_get_community_matches(mvgpu_ctx *ctx, int64_t *size, int64_t *best, int64_t *overlap, int64_t *best_size);
 
-/* currComm of this rank's vertices at exit (global community ids), lnv entries. */
+/* currComm of this rank's vertices at exit (global community ids), lnv entries, of the last mvgpu_louvain on the current
+ * shard: it fails with "no run on this shard" after an upload / attach / generate until the new shard's first run;
+ * mvgpu_update_shard keeps serving the last run's result. */
 int mvgpu_get_communities(mvgpu_ctx *ctx, int64_t *out);
-/* Same values left in device memory (int32 global ids); valid until the next mvgpu_louvain. */
+/* Same values left in device memory (int32 global ids), same contract; valid until the next mvgpu_louvain. */
 int mvgpu_get_communities_device(mvgpu_ctx *ctx, const int32_t **d_out);
 
 /* Options: "trace" (0/1: record moved/chash per iteration, default 0), "max_iters" (safety cap,
@@ -258,16 +274,19 @@ int mvgpu_get_communities_device(mvgpu_ctx *ctx, const int32_t **d_out);
  * after iteration k; if the exit test fires first the run ends as without it, see mvgpu_get_converged), "frontier" (0
  * (default) / 1: grow the movable set from the vertices that move, see mvgpu_set_movable; no effect without a set).
  * The environment variable MVGPU_OPTIONS="name=value,name=value" presets options for every context of the process. */
-/* In a multi-rank run every rank must set the same options (they change which collectives a run issues). */
+/* In a multi-rank run every rank must set the same options (they change which collectives a run issues).  A refused
+ * value or an unknown name changes nothing. */
 int mvgpu_set_option(mvgpu_ctx *ctx, const char *name, int64_t value);
+/* mvgpu_get_trace, mvgpu_get_timings, mvgpu_get_scan_times, mvgpu_get_constant and mvgpu_get_converged describe the last
+ * mvgpu_louvain call, whatever shard the context holds now. */
 int mvgpu_get_trace(mvgpu_ctx *ctx, int max_entries, mvgpu_iter_trace *out, int *n);
 int mvgpu_get_timings(mvgpu_ctx *ctx, mvgpu_timings *out);
 /* Device time (seconds) of the neighbour-scan launch(es) of each iteration of the last run; *n = #iterations. */
 int mvgpu_get_scan_times(mvgpu_ctx *ctx, int max_entries, double *out, int *n);
 /* 1/(2m), the reference's constantForSecondTerm (dspl.hpp:129), of the last run. */
 int mvgpu_get_constant(mvgpu_ctx *ctx, double *out);
-/* Shard statistics after upload/louvain: info[0]=lnv, [1]=lne, [2]=nghost, [3]=send list length,
- * [4]=#high-degree vertices, [5]=max degree. */
+/* Shard statistics: info[0]=lnv, [1]=lne of the current shard; from the setup of the last run on it (0 until its first
+ * run): [2]=nghost, [3]=send list length, [4]=#high-degree vertices, [5]=max degree. */
 int mvgpu_get_shard_info(mvgpu_ctx *ctx, int64_t *info6);
 
 /* ---- one-call form of the reference seam ------------------------------------------------------ */
@@ -284,6 +303,7 @@ int mvgpu_upload_shard32(mvgpu_ctx *ctx, int32_t nv_global, const int32_t *parts
                          const int32_t *edge_indices, const void *edge_list8);
 /* Fails while an initial assignment or "stop_after" is set (warm start is a 64-bit surface feature). */
 int mvgpu_louvain32(mvgpu_ctx *ctx, float lower, float thresh, int *iters, float *modularity);
+/* The contract of mvgpu_get_communities. */
 int mvgpu_get_communities32(mvgpu_ctx *ctx, int32_t *out);
 
 /* distLouvainMethod(me, nprocs, g, ..., lower, thresh, iters) for a single-GPU run with HOST arrays:

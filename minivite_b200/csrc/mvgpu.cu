@@ -268,6 +268,8 @@ struct mvgpu_ctx {
   double constant = 0.0;
   int32_t *d_final = nullptr;          // currComm at exit (points into comm_a/comm_b)
   bool final_ready = false;            // final_orig holds the assignment of the last run in the caller's numbering
+  bool final_on_shard = false;         // d_final / final_orig describe the current shard's vertices (update_shard keeps it,
+                                       // a shard replacement clears it): what the per-vertex result getters serve
   std::vector<mvgpu_iter_trace> trace;
   std::vector<double> scan_times;
   mvgpu_timings tm;
@@ -380,33 +382,46 @@ int coll_barrier(mvgpu_ctx *c) {
   return coll_sync(c);
 }
 
+// what is wrong with a shard description ("" if nothing); reads nothing of the context but its rank identity
+std::string check_graph(const mvgpu_ctx *c, long long nv_global, const int64_t *parts, long long lnv, long long lne) {
+  if (c->nranks > kMaxRanks) return "too many ranks";
+  if (nv_global < 0 || lnv < 0 || lne < 0) return "negative graph size";
+  if (nv_global >= (1LL << 31)) return "nv_global >= 2^31: 32-bit community ids would overflow (not supported)";
+  if (lne >= (1LL << 32)) return "lne >= 2^32 per shard: 32-bit edge offsets would overflow (not supported)";
+  if (parts[0] != 0 || parts[c->nranks] != nv_global) return "parts[] must run from 0 to nv_global";
+  for (int r = 0; r < c->nranks; r++) if (parts[r + 1] < parts[r]) return "parts[] not monotone";
+  if (parts[c->rank + 1] - parts[c->rank] != lnv) return "lnv does not match parts[rank+1]-parts[rank]";
+  return "";
+}
+
+// The shard is replaced: validated first, so that a refusal changes nothing.  From here on the context has no shard
+// until set_source names the new arrays -- a failure in between leaves it without one, and every compute entry point
+// refuses (check_ready).
 int set_graph(mvgpu_ctx *c, long long nv_global, const int64_t *parts, long long lnv, long long lne) {
-  if (c->nranks > kMaxRanks) return fail("too many ranks");
+  const std::string err = check_graph(c, nv_global, parts, lnv, lne);
+  if (!err.empty()) return fail(err);
   c->have_init = false;                     // an initial assignment belongs to the shard it was given for
   c->have_mov = c->mov_out_valid = false;   // and so does a movable set
   c->run_on_shard = c->eval_on_shard = false;   // so do a run's assignment and an evaluation
   c->cmp_on_shard = false;                      // and a comparison's matches
-  if (nv_global < 0 || lnv < 0 || lne < 0) return fail("negative graph size");
-  if (nv_global >= (1LL << 31)) return fail("nv_global >= 2^31: 32-bit community ids would overflow (not supported)");
-  if (lne >= (1LL << 32)) return fail("lne >= 2^32 per shard: 32-bit edge offsets would overflow (not supported)");
+  c->final_on_shard = c->final_ready = false;   // and the result the per-vertex getters serve
   c->parts.assign(parts, parts + c->nranks + 1);
-  if (c->parts[0] != 0 || c->parts[c->nranks] != nv_global) return fail("parts[] must run from 0 to nv_global");
-  for (int r = 0; r < c->nranks; r++) if (c->parts[r + 1] < c->parts[r]) return fail("parts[] not monotone");
   c->base = c->parts[c->rank];
   c->bound = c->parts[c->rank + 1];
-  if (c->bound - c->base != lnv) return fail("lnv does not match parts[rank+1]-parts[rank]");
   c->nv_global = nv_global; c->lnv = lnv; c->lne = lne;
-  c->have_graph = true;
+  c->have_graph = false;
   c->peers_ready = false;
   c->d_rowptr64 = nullptr; c->d_edges = nullptr; c->d_tails32 = nullptr;   // set_source names the new shard's arrays
   return 0;
 }
 
-// where setup_run reads the shard set_graph described (full records or compact tails) and what uploading it cost
+// where setup_run reads the shard set_graph described (full records or compact tails) and what uploading it cost; the
+// context has a shard from here on
 void set_source(mvgpu_ctx *c, const long long *rowptr64, const Edge16 *edges, const int32_t *tails32, bool f32, double h2d_s,
                 long long h2d_bytes) {
   c->d_rowptr64 = rowptr64; c->d_edges = edges; c->d_tails32 = tails32; c->f32 = f32;
   c->h2d_s = h2d_s; c->h2d_bytes = h2d_bytes;
+  c->have_graph = true;
 }
 
 // CUB's two-phase protocol for one or more calls that share c->cub_tmp: every size query, one (grow-only) ensure of the
@@ -664,9 +679,24 @@ int input_pass(mvgpu_ctx *c, const EvalSetup *ev, Scalars &h, int &unit, std::st
   return 0;
 }
 
+// The partition agreement rides on a sum all-reduce: slot r carries rank r's fingerprint of (nv_global, parts) and every
+// other rank contributes 0 there, so after the sum every rank holds every rank's fingerprint and reaches the same verdict.
+const char *const kPartitionDisagree = "ranks disagree on the partition: every rank must hold a shard of the same nv_global and parts";
+void partition_slots(const mvgpu_ctx *c, long long *slots) {
+  unsigned long long h = 0xcbf29ce484222325ULL ^ (unsigned long long)c->nv_global;
+  for (long long p : c->parts) h = (h ^ (unsigned long long)p) * 0x100000001b3ULL;   // FNV-1a over the offsets
+  h ^= h >> 29;
+  for (int r = 0; r < c->nranks; r++) slots[r] = 0;
+  slots[c->rank] = (long long)(h >> 1);                  // non-negative: a sum of one of them and zeros cannot overflow
+}
+bool partition_agrees(const mvgpu_ctx *c, const long long *slots) {
+  for (int r = 1; r < c->nranks; r++) if (slots[r] != slots[0]) return false;
+  return true;
+}
+
 // The one setup agreement (one all-reduce): path, edge total, input errors, "must grow an exported array", "was given
-// an assignment".  Errors are agreed on before anybody returns: a rank that left alone would leave its peers blocked in
-// the next collective.  Sets c->unit (2m < 2^31 settles from the edge total; the weight total comes later).
+// an assignment", the partition.  Errors are agreed on before anybody returns: a rank that left alone would leave its
+// peers blocked in the next collective.  Sets c->unit (2m < 2^31 settles from the edge total; the weight total comes later).
 int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, std::string err) {
   long long ne_global = c->lne;
   if (c->nranks > 1) {
@@ -677,12 +707,15 @@ int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, 
     bool grow = false;
     for (const Export &e : x) grow = grow || (c->ipc_valid && e.cap && e.cap < e.need);
     const bool assigned = ev ? ev->given : c->warm_run;
-    // [5], [6]: a movable set, and its frontier option (a rank would store into a peer's unexported next set)
-    long long hv[7] = {unit ? 0 : 1, c->lne, err.empty() ? 0 : 1, grow ? 1 : 0, assigned ? 1 : 0, c->mov_run ? 1 : 0,
-                       c->mov_run && c->opt_frontier ? 1 : 0};
-    TRY(coll_allreduce_i64(c, hv, 7, false));
+    // [5], [6]: a movable set, and its frontier option (a rank would store into a peer's unexported next set);
+    // [7 + r]: rank r's partition fingerprint
+    long long hv[7 + kMaxRanks] = {unit ? 0 : 1, c->lne, err.empty() ? 0 : 1, grow ? 1 : 0, assigned ? 1 : 0, c->mov_run ? 1 : 0,
+                                   c->mov_run && c->opt_frontier ? 1 : 0};
+    partition_slots(c, hv + 7);
+    TRY(coll_allreduce_i64(c, hv, 7 + c->nranks, false));
     unit = hv[0] == 0;
     ne_global = hv[1];
+    if (err.empty() && !partition_agrees(c, hv + 7)) err = kPartitionDisagree;
     if (hv[2] && err.empty()) err = ev ? "another rank rejected its shard or its assignment" : "another rank rejected its shard";
     if (err.empty() && hv[4] != 0 && hv[4] != c->nranks)
       err = ev ? (ev->split ? "ranks disagree on the assignment to split: every rank or none must pass NULL"
@@ -1014,6 +1047,13 @@ int setup_run(mvgpu_ctx *c, const EvalSetup *ev = nullptr) {
   TRY(renumber(c, ev, g));
   c->a_rowptr = g.rowptr; c->a_tails = g.tails; c->a_weights = g.weights;
   TRY(init_state(c, ev, nremote));
+  if (!ev) {
+    // The arrays the run writes after its last iteration are sized here, before the first peer-memory collective: a
+    // grow there frees the old block, and cudaFree waits for the whole device -- including a peer rank's barrier kernel
+    // that spins until this rank's barrier arrives (ranks sharing a device would wait on each other until the watchdog).
+    TRY(c->final_orig.ensure(c->lnv));
+    if (c->mov_run) TRY(c->mov_out.ensure(c->lnv));
+  }
   long long heavy_deg = 0;
   TRY(heavy_launch(c, heavy_deg));
   TRY(total_weight(c, h));
@@ -1045,7 +1085,7 @@ int exchange_ghosts(mvgpu_ctx *c, int32_t *comm) {
 
 // a graph and, with several ranks, a communicator that carries the run's data plane
 int check_ready(mvgpu_ctx *c) {
-  if (!c->have_graph) return fail("no graph uploaded");
+  if (!c->have_graph || !c->d_rowptr64) return fail("no graph uploaded");
   if (c->nranks > 1 && !c->comm && !c->hc.is_open()) return fail("mvgpu_comm_init has not been called");
   if (c->nranks > 1 && !c->comm && c->opt_comm_mode != 1) return fail("comm_mode=0 (NCCL data plane) needs the NCCL communicator: host_transport=1 supports comm_mode=1 only");
   return 0;
@@ -1232,10 +1272,9 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   CK(cudaEventRecord(e_end, s));
   c->d_final = cur;
   c->final_ready = false;
-  c->run_on_shard = true;
+  c->run_on_shard = c->final_on_shard = true;
   if (c->mov_run) {                                            // M_{k+1} in caller numbering, outside the timed region
-    TRY(c->mov_out.ensure(c->lnv));
-    if (c->lnv > 0) {
+    if (c->lnv > 0) {                                          // mov_out was sized in setup_run
       k_movable_out<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, s>>>((int)c->lnv, mov[k_cur], c->relabel ? c->inv.p : nullptr, c->mov_out.p);
       CK(cudaGetLastError());
     }
@@ -1749,8 +1788,10 @@ int compare(mvgpu_ctx *c, const int64_t *x, const int64_t *y, mvgpu_compare_repo
   // the call's first collective: one rank's finding fails every rank before any data moves
   if (c->nranks > 1) {
     TRY(c->scratch.ensure(sizeof(Scalars)));
-    long long hv[2] = {err.empty() ? 0 : 1, x ? 1 : 0};
-    TRY(coll_allreduce_i64(c, hv, 2, false));
+    long long hv[2 + kMaxRanks] = {err.empty() ? 0 : 1, x ? 1 : 0};
+    partition_slots(c, hv + 2);
+    TRY(coll_allreduce_i64(c, hv, 2 + c->nranks, false));
+    if (err.empty() && !partition_agrees(c, hv + 2)) err = who + ": " + kPartitionDisagree;
     if (hv[0] && err.empty()) err = who + ": another rank rejected its assignment";
     if (err.empty() && hv[1] != 0 && hv[1] != c->nranks)
       err = who + ": ranks disagree on the assignment x: every rank or none must pass NULL";
@@ -1865,9 +1906,9 @@ int update_prepare(mvgpu_ctx *c, long long n_del, const int64_t *del_src, const 
 // =================================================================================================
 // `-p`: random long edges on top of the generated strip (graph.hpp:939-1122; host/rgg.hpp add_random_edges is the
 // restatement this follows, including its fixed seed).  Every rank replays all p draw streams (they are cheap and
-// sequential) and keeps the records that touch its strip.
+// sequential) and keeps the records that touch its strip.  rowptr / edges: the strip being built (replaced by the merge).
 static int add_random_edges(mvgpu_ctx *c, const RggParams &P, int64_t nv, int unit, double pct, const double *X3, const double *Y3,
-                            long long *lne_io) {
+                            DevBuf<long long> &rowptr, DevBuf<Edge16> &edges, long long *lne_io) {
   const int p = c->nranks, nsm = c->num_sms;
   cudaStream_t s = c->stream;
   if (nv >= 2147483645LL) return fail("random edges: nv too large for the device generator");
@@ -1895,7 +1936,7 @@ static int add_random_edges(mvgpu_ctx *c, const RggParams &P, int64_t nv, int un
   TRY(emit.ensure(nrande + 1)); TRY(epos.ensure(nrande + 1));
   CK(cudaMemcpyAsync(dsoff.p, soff.data(), sizeof(long long) * (p + 1), cudaMemcpyHostToDevice, s));
   k_rande_draws<<<p, 32, 0, s>>>(R, dsoff.p, di.p, dgj.p);
-  k_rande_keys<<<grid_for(nrande, 256, nsm), 256, 0, s>>>(R, dsoff.p, di.p, dgj.p, nrande, c->gen_rowptr.p, c->gen_edges.p, key.p, qidx.p);
+  k_rande_keys<<<grid_for(nrande, 256, nsm), 256, 0, s>>>(R, dsoff.p, di.p, dgj.p, nrande, rowptr.p, edges.p, key.p, qidx.p);
   TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, key.p, skey.p, qidx.p, sq.p, (int)nrande, 0, 64, s); }));
   CK(cudaMemsetAsync(emit.p + nrande, 0, sizeof(unsigned int), s));
   k_rande_first<<<grid_for(nrande, 256, nsm), 256, 0, s>>>(skey.p, sq.p, nrande, R, dsoff.p, dgj.p, emit.p);
@@ -1911,9 +1952,9 @@ static int add_random_edges(mvgpu_ctx *c, const RggParams &P, int64_t nv, int un
   // the extras are an insert-only batch in push order: merged like an update, RGG records first among equal tails
   DevBuf<Edge16> merged;
   long long lne2 = 0;
-  TRY(merge_records(c, P.n, c->gen_rowptr.p, c->gen_edges.p, *lne_io, nullptr, 0, sxkey.p, sxidx.p, xw.p, nextra, nrow, merged, &lne2));
-  c->gen_edges.swap(merged);
-  c->gen_rowptr.swap(nrow);
+  TRY(merge_records(c, P.n, rowptr.p, edges.p, *lne_io, nullptr, 0, sxkey.p, sxidx.p, xw.p, nextra, nrow, merged, &lne2));
+  edges.swap(merged);
+  rowptr.swap(nrow);
   *lne_io = lne2;
   return 0;
 }
@@ -2243,6 +2284,10 @@ int mvgpu_generate_rgg_shard_ex(mvgpu_ctx *c, int64_t nv_global, int unit_weight
   DevBuf<double> X, UY, cx, cy;                        // X, UY: coordinates of up to three strips (own + neighbours)
   DevBuf<long long> cgid, deg;
   DevBuf<unsigned int> cnt, cstart;
+  // the new strip is built in its own arrays: the current shard (possibly the last generated one) stays intact until
+  // everything that can refuse has passed
+  DevBuf<long long> rowptr;
+  DevBuf<Edge16> edges;
   TRY(X.ensure(3 * P.n)); TRY(UY.ensure(3 * P.n)); TRY(cnt.ensure(ncells + 1)); TRY(cstart.ensure(ncells + 1)); TRY(deg.ensure(P.n + 1));
   k_rgg_points<<<grid_for(P.n, 256, nsm), 256, 0, s>>>(P, X.p, UY.p);
   CK(cudaMemsetAsync(cnt.p, 0, sizeof(unsigned int) * (ncells + 1), s));
@@ -2256,21 +2301,23 @@ int mvgpu_generate_rgg_shard_ex(mvgpu_ctx *c, int64_t nv_global, int unit_weight
   k_rgg_bin<<<grid_for(P.n, 256, nsm), 256, 0, s>>>(P, X.p, UY.p, 1, cnt.p, cstart.p, cx.p, cy.p, cgid.p);
   CK(cudaMemsetAsync(deg.p + P.n, 0, sizeof(long long), s));
   k_rgg_neighbours<false><<<grid_for(P.n, 128, nsm, 16), 128, 0, s>>>(P, X.p, UY.p, cstart.p, cx.p, cy.p, cgid.p, unit_weight, deg.p, nullptr);
-  TRY(c->gen_rowptr.ensure(P.n + 1));
-  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, deg.p, c->gen_rowptr.p, (int)(P.n + 1), s); }));
+  TRY(rowptr.ensure(P.n + 1));
+  TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceScan::ExclusiveSum(t, tb, deg.p, rowptr.p, (int)(P.n + 1), s); }));
   long long lne = 0;
-  CK(cudaMemcpyAsync(&lne, c->gen_rowptr.p + P.n, sizeof lne, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&lne, rowptr.p + P.n, sizeof lne, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  TRY(c->gen_edges.ensure(lne));
-  k_rgg_neighbours<true><<<grid_for(P.n, 128, nsm, 16), 128, 0, s>>>(P, X.p, UY.p, cstart.p, cx.p, cy.p, cgid.p, unit_weight, c->gen_rowptr.p, c->gen_edges.p);
+  TRY(edges.ensure(lne));
+  k_rgg_neighbours<true><<<grid_for(P.n, 128, nsm, 16), 128, 0, s>>>(P, X.p, UY.p, cstart.p, cx.p, cy.p, cgid.p, unit_weight, rowptr.p, edges.p);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(s));
   cx.release(); cy.release(); cgid.release(); deg.release(); cnt.release(); cstart.release();
-  if (random_edge_percent > 0.0) TRY(add_random_edges(c, P, nv_global, unit_weight, random_edge_percent, X.p, UY.p, &lne));
+  if (random_edge_percent > 0.0) TRY(add_random_edges(c, P, nv_global, unit_weight, random_edge_percent, X.p, UY.p, rowptr, edges, &lne));
   X.release(); UY.release();
   std::vector<int64_t> parts(p + 1);
   for (int q = 0; q <= p; q++) parts[q] = (nv_global * q) / p;
-  TRY(set_graph(c, nv_global, parts.data(), P.n, lne));
+  TRY(set_graph(c, nv_global, parts.data(), P.n, lne));   // validates before it changes anything
+  c->gen_rowptr.swap(rowptr);                              // the old generated arrays, if any, go with the temporaries
+  c->gen_edges.swap(edges);
   set_source(c, c->gen_rowptr.p, c->gen_edges.p, nullptr, false, 0.0, 0);
   if (lne_out) *lne_out = lne;
   return 0;
@@ -2350,10 +2397,10 @@ int mvgpu_set_initial_communities(mvgpu_ctx *c, const int64_t *comm) {
 
 int mvgpu_set_movable(mvgpu_ctx *c, const uint8_t *mask) {
   if (!c) return fail("null argument");
+  if (mask && !c->have_graph) return fail("mvgpu_set_movable: no shard yet (upload, attach or generate one first)");
   c->mov_out_valid = false;
   c->peers_ready = false;          // a masked run with the frontier option exports two more arrays
   if (!mask) { c->have_mov = false; return 0; }
-  if (!c->have_graph) return fail("mvgpu_set_movable: no shard yet (upload, attach or generate one first)");
   CK(cudaSetDevice(c->device));
   TRY(c->mov_in.ensure(c->lnv));
   if (c->lnv) {                                // on the context's stream, behind any run still reading mov_in
@@ -2459,8 +2506,12 @@ int mvgpu_get_converged(mvgpu_ctx *c, int *converged) {
   return 0;
 }
 
+// the per-vertex result getters serve the last run on the current shard (mvgpu_update_shard keeps it)
+const char *const kNoRunOnShard = "no run on this shard yet (mvgpu_louvain after the last upload / attach / generate)";
+
 int mvgpu_get_communities_device(mvgpu_ctx *c, const int32_t **d_out) {
-  if (!c || !c->d_final) return fail("no result yet");
+  if (!c || !d_out) return fail("null argument");
+  if (!c->final_on_shard) return fail(kNoRunOnShard);
   TRY(final_in_caller_order(c));
   CK(cudaStreamSynchronize(c->stream));
   *d_out = c->final_orig.p;
@@ -2468,7 +2519,8 @@ int mvgpu_get_communities_device(mvgpu_ctx *c, const int32_t **d_out) {
 }
 
 int mvgpu_get_communities(mvgpu_ctx *c, int64_t *out) {
-  if (!c || !c->d_final) return fail("no result yet");
+  if (!c || !out) return fail("null argument");
+  if (!c->final_on_shard) return fail(kNoRunOnShard);
   if (c->lnv == 0) return 0;
   TRY(final_in_caller_order(c));
   TRY(c->wide.ensure(c->lnv));
@@ -2507,10 +2559,8 @@ int mvgpu_get_communities(mvgpu_ctx *c, int64_t *out) {
   return 0;
 }
 
-int mvgpu_set_option(mvgpu_ctx *c, const char *name, int64_t value) {
-  if (!c || !name) return fail("null argument");
-  const std::string n(name);
-  c->peers_ready = false;          // options may change which arrays exist: re-validate the peer tables
+// one option; a refusal changes nothing
+static int set_option_value(mvgpu_ctx *c, const std::string &n, int64_t value) {
   if (n == "trace") c->opt_trace = value != 0;
   else if (n == "max_iters") { if (value < 1) return fail("max_iters < 1"); c->opt_max_iters = value; }
   else if (n == "force_weighted") c->opt_force_weighted = value != 0;
@@ -2532,6 +2582,13 @@ int mvgpu_set_option(mvgpu_ctx *c, const char *name, int64_t value) {
   }
   else if (n == "region_size") { if (value < 32) return fail("region_size < 32"); c->opt_region = (int)value; }
   else return fail("unknown option " + n);
+  return 0;
+}
+
+int mvgpu_set_option(mvgpu_ctx *c, const char *name, int64_t value) {
+  if (!c || !name) return fail("null argument");
+  TRY(set_option_value(c, name, value));
+  c->peers_ready = false;          // options may change which arrays exist: re-validate the peer tables
   return 0;
 }
 
@@ -2565,7 +2622,9 @@ int mvgpu_get_constant(mvgpu_ctx *c, double *out) {
 
 int mvgpu_get_shard_info(mvgpu_ctx *c, int64_t *info6) {
   if (!c || !info6) return fail("null argument");
-  info6[0] = c->lnv; info6[1] = c->lne; info6[2] = c->nghost; info6[3] = c->nsend; info6[4] = c->nheavy; info6[5] = c->maxdeg;
+  const bool ran = c->final_on_shard;          // [2..5] come from a run's setup: 0 until the shard's first run
+  info6[0] = c->lnv; info6[1] = c->lne; info6[2] = ran ? c->nghost : 0; info6[3] = ran ? c->nsend : 0;
+  info6[4] = ran ? c->nheavy : 0; info6[5] = ran ? c->maxdeg : 0;
   return 0;
 }
 
@@ -2578,7 +2637,9 @@ int mvgpu_get_shard_info(mvgpu_ctx *c, int64_t *info6) {
 int mv_layout_readback(mvgpu_ctx *c, int64_t *info16, uint32_t *rowptr, int32_t *tails, uint32_t *bfs_key, int32_t *perm,
                        int32_t *inv, int32_t *lab, uint32_t *rowptr2, int32_t *tails2, double *weights2) {
   if (!c) return fail("null ctx");
-  if (!c->d_final) return fail("no run yet");
+  // keyed on run_on_shard, not final_on_shard: the arrays it returns are the last run's compact CSR, sized by that
+  // run's lne, so it refuses after mvgpu_update_shard too (the per-vertex labels stay valid there, the CSR does not)
+  if (!c->run_on_shard) return fail("no run on this shard yet: mv_layout_readback describes the last mvgpu_louvain on the current shard");
   if (info16) {
     const int64_t v[16] = {c->lay.want, c->relabel, c->reordered ? 1 : 0, c->lay.stride, c->lay.nregions, c->lay.span[0],
                            c->lay.span[1], c->lay.unordered, c->lay.has_self, c->simple_sorted ? 1 : 0,
@@ -2644,7 +2705,8 @@ int mvgpu_louvain32(mvgpu_ctx *c, float lower, float thresh, int *iters, float *
 }
 
 int mvgpu_get_communities32(mvgpu_ctx *c, int32_t *out) {
-  if (!c || !c->d_final) return fail("no result yet");
+  if (!c || !out) return fail("null argument");
+  if (!c->final_on_shard) return fail(kNoRunOnShard);
   if (c->lnv == 0) return 0;
   TRY(final_in_caller_order(c));
   CK(cudaMemcpyAsync(out, c->final_orig.p, sizeof(int32_t) * c->lnv, cudaMemcpyDeviceToHost, c->stream));
