@@ -248,6 +248,9 @@ __device__ __forceinline__ double warp_sum(double v) {
 }
 
 // ---- helpers shared by the scan kernels ----------------------------------------------------------------
+// The per-vertex decision of distExecuteLouvainIteration (dspl.hpp:174-405), written once for k_scan_ws, k_scan_pw
+// and k_scan_pq (k_scan_heavy decides by a CTA-wide argmax and has its own).  Every sum and gain keeps the
+// reference's operation order, so each vertex decides as the reference does, bit for bit.
 template <bool MULTI>
 __device__ __forceinline__ void push_move_unit(const ScanParams &p, int cc, int best, int d) {
   atomicAdd(at_upd<MULTI>(p, best), pack_delta(1, (long long)d));
@@ -262,9 +265,160 @@ __device__ __forceinline__ void push_move_w(const ScanParams &p, int cc, int bes
   atomicAdd(at_udeg<MULTI>(p, cc), -vdeg);
 }
 
+// vertex v of degree d > 0 in community cc: degree of cc (a_x), its own degree (k_i) and its self-loop weight
+template <bool UNIT, bool MULTI>
+__device__ __forceinline__ void vertex_load(const ScanParams &p, int v, int cc, int d, double &cc_deg, double &vdeg,
+                                            double &sl) {
+  if (UNIT) {
+    cc_deg = (double)__ldg(at_cdeg<MULTI>(p, cc));
+    vdeg = (double)d;
+    sl = p.has_self ? (double)__ldg(p.self_i + v) : 0.0;
+  } else {
+    cc_deg = __ldg(&at_cinfo_w<MULTI>(p, cc)->degree);
+    vdeg = __ldg(p.vdeg + v);
+    sl = p.has_self ? __ldg(p.self_d + v) : 0.0;
+  }
+}
+
+// pass 0 over the neighbour communities seg[0, d) (weights segw[0, d), not read when UNIT): w0 = weight towards the
+// own community cc, summed in edge order (counter[0], dspl.hpp:312-318).  The m other entries are compacted to the
+// front, stably, so edge order is kept.  Returns their number m; d - m edges lead into cc.
+template <bool UNIT>
+__device__ __forceinline__ int pass0(int32_t *seg, double *segw, int d, int cc, double &w0) {
+  int m = 0;
+  w0 = 0.0;
+  for (int k = 0; k < d; k++) {
+    const int x = seg[k];
+    if (x == cc) { if (!UNIT) w0 += segw[k]; }
+    else {
+      seg[m] = x;
+      if (!UNIT) segw[m] = segw[k];
+      m++;
+    }
+  }
+  if (UNIT) w0 = (double)(d - m);
+  return m;
+}
+
+// pass 1 over the m entries pass 0 left: two distinct neighbour communities per lane per round.  The round's walk
+// counts the community of the first live entry and the first community that differs from it, and compacts everything
+// else to the front, so the live list only ever shrinks and no lane has to skip over already counted entries.  Each
+// sum is accumulated in segment order, i.e. edge order, which keeps the weighted path's rounding the reference's.  The
+// community degree gather issued before the walk is consumed after it.  best/lbest come in as the current community /
+// kNoLabel and leave as the winner under dspl.hpp:214-215 and its cached label.
+// All 32 lanes of the warp must call it (__any_sync); a lane without work passes m = 0.
+template <bool UNIT, bool MULTI>
+__device__ __forceinline__ void pass1(const ScanParams &p, int32_t *seg, double *segw, int m, double eix, double vdeg,
+                                      double ax, int &best, int &lbest) {
+  double bg = 0.0;
+  for (;;) {
+    const bool has = m > 0;
+    if (!__any_sync(0xffffffffu, has)) break;
+    int ck1 = 0;
+    double ay1 = 0.0;
+    if (has) {
+      ck1 = seg[0];
+      if (UNIT) ay1 = (double)__ldg(at_cdeg<MULTI>(p, ck1));
+      else ay1 = __ldg(&at_cinfo_w<MULTI>(p, ck1)->degree);
+    }
+    int ck2 = -1, c1 = 0, c2 = 0, m2 = 0;
+    double sum1 = 0.0, sum2 = 0.0;
+    for (int j = 0; j < m; j++) {
+      const int x = seg[j];
+      if (x == ck1) { if (UNIT) c1++; else sum1 += segw[j]; }
+      else {
+        if (ck2 < 0) ck2 = x;
+        if (x == ck2) { if (UNIT) c2++; else sum2 += segw[j]; }
+        else {
+          seg[m2] = x;
+          if (!UNIT) segw[m2] = segw[j];
+          m2++;
+        }
+      }
+    }
+    m = m2;
+    if (has) {
+      if (UNIT) sum1 = (double)c1;
+      const double g1 = gain_of(sum1, eix, vdeg, ay1, ax, p.constant, p.f32);
+      if (better_l<MULTI>(p, g1, ck1, bg, best, lbest)) { bg = g1; best = ck1; }
+      if (ck2 >= 0) {
+        double ay2;
+        if (UNIT) { ay2 = (double)__ldg(at_cdeg<MULTI>(p, ck2)); sum2 = (double)c2; }
+        else ay2 = __ldg(&at_cinfo_w<MULTI>(p, ck2)->degree);
+        const double g2 = gain_of(sum2, eix, vdeg, ay2, ax, p.constant, p.f32);
+        if (better_l<MULTI>(p, g2, ck2, bg, best, lbest)) { bg = g2; best = ck2; }
+      }
+    }
+  }
+}
+
+// singleton veto (dspl.hpp:224-225) for vertex of degree d: a singleton does not move to a singleton of larger label.
+// Returns the community the vertex ends in.  The test of d only skips the label lookup: d == 0 leaves best == cc,
+// where label_greater is false.
+template <bool UNIT, bool MULTI>
+__device__ __forceinline__ int singleton_veto(const ScanParams &p, int cc, int best, int lbest, int d) {
+  if (d && label_greater<MULTI>(p, best, lbest, cc)) {
+    long long sz_cc, sz_b;
+    if (UNIT) {
+      sz_cc = __ldg(at_csize<MULTI>(p, cc));
+      sz_b = __ldg(at_csize<MULTI>(p, best));
+    } else {
+      sz_cc = __ldg(&at_cinfo_w<MULTI>(p, cc)->size);
+      sz_b = __ldg(&at_cinfo_w<MULTI>(p, best)->size);
+    }
+    if (sz_cc == 1 && sz_b == 1) return cc;
+  }
+  return best;
+}
+
+// the move of vertex v from cc to best as community deltas (dspl.hpp:331-399), and its trace terms.  The caller
+// stores targetComm (dspl.hpp:404) itself, with its own cache policy.  vdeg is read on the weighted path only.
+template <bool UNIT, bool MULTI, bool TRACE>
+__device__ __forceinline__ void commit(const ScanParams &p, int v, int cc, int best, int d, double vdeg,
+                                       unsigned long long &acc_moved, unsigned long long &acc_hash) {
+  if (best != cc) {
+    if (UNIT) push_move_unit<MULTI>(p, cc, best, d);
+    else push_move_w<MULTI>(p, cc, best, vdeg);
+  }
+  if (TRACE) { acc_moved += (best != cc); acc_hash += vhash(label_of<MULTI>(p, (int)(p.base + v)), label_of<MULTI>(p, best)); }
+}
+
+// end of a scan kernel: the CTA's NWARPS warps add their accumulators up and thread 0 issues one atomic per field
+template <bool UNIT, bool TRACE, int NWARPS>
+__device__ __forceinline__ void flush_acc(const ScanParams &p, unsigned long long le_u, double le_d,
+                                          unsigned long long moved, unsigned long long hash) {
+  __shared__ unsigned long long s_red[3][NWARPS];
+  __shared__ double s_redd[NWARPS];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (UNIT) { const unsigned long long s = warp_sum(le_u); if (lane == 0) s_red[0][wid] = s; }
+  else { const double s = warp_sum(le_d); if (lane == 0) s_redd[wid] = s; }
+  if (TRACE) {
+    const unsigned long long a = warp_sum(moved), b = warp_sum(hash);
+    if (lane == 0) { s_red[1][wid] = a; s_red[2][wid] = b; }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (UNIT) {
+      unsigned long long s = 0;
+      for (int w = 0; w < NWARPS; w++) s += s_red[0][w];
+      if (s) atomicAdd(&p.acc->le_u, s);
+    } else {
+      double s = 0;
+      for (int w = 0; w < NWARPS; w++) s += s_redd[w];
+      if (s != 0.0) atomicAdd(&p.acc->le_d, s);
+    }
+    if (TRACE) {
+      unsigned long long a = 0, b = 0;
+      for (int w = 0; w < NWARPS; w++) { a += s_red[1][w]; b += s_red[2][w]; }
+      atomicAdd(&p.acc->moved, a);
+      atomicAdd(&p.acc->hash, b);
+    }
+  }
+}
+
 // ----------------------------------------------------------------------------------------------
 // Neighbour-scan kernel, second generation ("warp-synchronous loops"; option scan_variant=3, the default of round 1;
-// the default is now k_scan_pw in scan_pipe.cuh, which keeps this kernel's phase B):
+// the default is now k_scan_pw in scan_pipe.cuh, which shares this kernel's phase B through the helpers above):
 // distExecuteLouvainIteration + distBuildLocalMapCounter + distGetMaxIndex (dspl.hpp:276-405, 230-274, 174-228).
 // One CTA owns a tile of kTileV (128) consecutive vertices; their CSR edges are one contiguous range.
 //   phase A (edge-parallel, all lanes busy, coalesced): stream the int32 tails of the tile, gather cur[tail] (the only
@@ -292,8 +446,6 @@ __global__ void __launch_bounds__(kTileV) k_scan_ws(const ScanParams p, const ui
   double *s_w = reinterpret_cast<double *>(smem_raw + sizeof(int32_t) * kECap);
   __shared__ int s_next, s_end, s_skip;
   __shared__ uint32_t s_e0;
-  __shared__ unsigned long long s_red[3][kTileV / 32];
-  __shared__ double s_redd[kTileV / 32];
 
   const int tid = threadIdx.x;
   const int v0 = blockIdx.x * kTileV;
@@ -353,126 +505,23 @@ __global__ void __launch_bounds__(kTileV) k_scan_ws(const ScanParams p, const ui
     int cc = 0, best = 0;
     if (mine) { cc = __ldg(p.cur + v); best = cc; }
     double cc_deg = 0.0, vdeg = 0.0, sl = 0.0;
-    if (d) {
-      if (UNIT) {
-        cc_deg = (double)__ldg(at_cdeg<MULTI>(p, cc));
-        vdeg = (double)d;
-        sl = p.has_self ? (double)__ldg(p.self_i + v) : 0.0;
-      } else {
-        cc_deg = __ldg(&at_cinfo_w<MULTI>(p, cc)->degree);
-        vdeg = __ldg(p.vdeg + v);
-        sl = p.has_self ? __ldg(p.self_d + v) : 0.0;
-      }
-    }
-    // pass 0: weight towards the own community, in edge order (counter[0], dspl.hpp:312-318); the other
-    // neighbours are compacted to the front of the segment (stable, so edge order is kept)
-    double w0 = 0.0;
-    int cnt0 = 0, m = 0;
-    for (int k = 0; k < d; k++) {
-      const int x = s_comm[o0 + k];
-      if (x == cc) { if (UNIT) cnt0++; else w0 += s_w[o0 + k]; }
-      else {
-        s_comm[o0 + m] = x;
-        if (!UNIT) s_w[o0 + m] = s_w[o0 + k];
-        m++;
-      }
-    }
-    if (UNIT) w0 = (double)cnt0;
+    if (d) vertex_load<UNIT, MULTI>(p, v, cc, d, cc_deg, vdeg, sl);
+    double w0;
+    int m = pass0<UNIT>(s_comm + o0, s_w + o0, d, cc, w0);
     const double eix = __dsub_rn(w0, sl), ax = __dsub_rn(cc_deg, vdeg);
-    if (d) { if (UNIT) acc_le_u += (unsigned long long)cnt0; else acc_le_d += w0; }
+    if (d) { if (UNIT) acc_le_u += (unsigned long long)(d - m); else acc_le_d += w0; }
     if (MASKED && d && !movable[v]) m = 0;                                 // frozen: no candidate, best stays cc
-    // pass 1: two distinct neighbour communities per lane per round.  The round's walk counts the community of the
-    // first live entry and the first community that differs from it, and compacts everything else to the front, so
-    // the live list only ever shrinks and no lane has to skip over already counted entries.
-    double bg = 0.0;
     int lbest = kNoLabel;
-    for (;;) {
-      const bool has = m > 0;
-      if (!__any_sync(0xffffffffu, has)) break;
-      int ck1 = 0;
-      double ay1 = 0.0;
-      if (has) {
-        ck1 = s_comm[o0];
-        if (UNIT) ay1 = (double)__ldg(at_cdeg<MULTI>(p, ck1));
-        else ay1 = __ldg(&at_cinfo_w<MULTI>(p, ck1)->degree);
-      }
-      int ck2 = -1, c1 = 0, c2 = 0, m2 = 0;
-      double sum1 = 0.0, sum2 = 0.0;
-      for (int j = 0; j < m; j++) {
-        const int x = s_comm[o0 + j];
-        if (x == ck1) { if (UNIT) c1++; else sum1 += s_w[o0 + j]; }
-        else {
-          if (ck2 < 0) ck2 = x;
-          if (x == ck2) { if (UNIT) c2++; else sum2 += s_w[o0 + j]; }
-          else {
-            s_comm[o0 + m2] = x;
-            if (!UNIT) s_w[o0 + m2] = s_w[o0 + j];
-            m2++;
-          }
-        }
-      }
-      m = m2;
-      if (has) {
-        if (UNIT) sum1 = (double)c1;
-        const double g1 = gain_of(sum1, eix, vdeg, ay1, ax, p.constant, p.f32);
-        if (better_l<MULTI>(p, g1, ck1, bg, best, lbest)) { bg = g1; best = ck1; }
-        if (ck2 >= 0) {
-          double ay2;
-          if (UNIT) { ay2 = (double)__ldg(at_cdeg<MULTI>(p, ck2)); sum2 = (double)c2; }
-          else ay2 = __ldg(&at_cinfo_w<MULTI>(p, ck2)->degree);
-          const double g2 = gain_of(sum2, eix, vdeg, ay2, ax, p.constant, p.f32);
-          if (better_l<MULTI>(p, g2, ck2, bg, best, lbest)) { bg = g2; best = ck2; }
-        }
-      }
-    }
+    pass1<UNIT, MULTI>(p, s_comm + o0, s_w + o0, m, eix, vdeg, ax, best, lbest);
     if (mine) {
-      if (d && label_greater<MULTI>(p, best, lbest, cc)) {                   // singleton veto, dspl.hpp:224-225
-        long long sz_cc, sz_b;
-        if (UNIT) {
-          sz_cc = __ldg(at_csize<MULTI>(p, cc));
-          sz_b = __ldg(at_csize<MULTI>(p, best));
-        } else {
-          sz_cc = __ldg(&at_cinfo_w<MULTI>(p, cc)->size);
-          sz_b = __ldg(&at_cinfo_w<MULTI>(p, best)->size);
-        }
-        if (sz_cc == 1 && sz_b == 1) best = cc;
-      }
-      if (best != cc) {                                                      // dspl.hpp:331-399
-        if (UNIT) push_move_unit<MULTI>(p, cc, best, d);
-        else push_move_w<MULTI>(p, cc, best, vdeg);
-      }
+      best = singleton_veto<UNIT, MULTI>(p, cc, best, lbest, d);
       st_pol(p.tgt + v, best, pol_str);                                      // dspl.hpp:404
-      if (TRACE) { acc_moved += (best != cc); acc_hash += vhash(label_of<MULTI>(p, (int)(p.base + v)), label_of<MULTI>(p, best)); }
+      commit<UNIT, MULTI, TRACE>(p, v, cc, best, d, vdeg, acc_moved, acc_hash);
     }
     start = end;
     __syncthreads();
   }
-
-  const int lane = tid & 31, wid = tid >> 5;
-  if (UNIT) { const unsigned long long s = warp_sum(acc_le_u); if (lane == 0) s_red[0][wid] = s; }
-  else { const double s = warp_sum(acc_le_d); if (lane == 0) s_redd[wid] = s; }
-  if (TRACE) {
-    const unsigned long long a = warp_sum(acc_moved), b = warp_sum(acc_hash);
-    if (lane == 0) { s_red[1][wid] = a; s_red[2][wid] = b; }
-  }
-  __syncthreads();
-  if (tid == 0) {
-    if (UNIT) {
-      unsigned long long s = 0;
-      for (int w = 0; w < kTileV / 32; w++) s += s_red[0][w];
-      if (s) atomicAdd(&p.acc->le_u, s);
-    } else {
-      double s = 0;
-      for (int w = 0; w < kTileV / 32; w++) s += s_redd[w];
-      if (s != 0.0) atomicAdd(&p.acc->le_d, s);
-    }
-    if (TRACE) {
-      unsigned long long a = 0, b = 0;
-      for (int w = 0; w < kTileV / 32; w++) { a += s_red[1][w]; b += s_red[2][w]; }
-      atomicAdd(&p.acc->moved, a);
-      atomicAdd(&p.acc->hash, b);
-    }
-  }
+  flush_acc<UNIT, TRACE, kTileV / 32>(p, acc_le_u, acc_le_d, acc_moved, acc_hash);
 }
 
 // ----------------------------------------------------------------------------------------------

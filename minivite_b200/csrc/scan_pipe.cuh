@@ -1,7 +1,8 @@
 // Neighbour-scan kernel, third generation: persistent warps fed by the TMA engine.
 //
-// Same arithmetic as k_scan_ws (kernels.cuh) -- distExecuteLouvainIteration + distBuildLocalMapCounter +
-// distGetMaxIndex, dspl.hpp:276-405, 230-274, 174-228 -- organised around what k_scan_ws's profile showed: it was
+// Same per-vertex decision as k_scan_ws, from the helpers shared by the scan kernels in kernels.cuh (pass0, pass1,
+// singleton_veto, commit) -- distExecuteLouvainIteration + distBuildLocalMapCounter + distGetMaxIndex,
+// dspl.hpp:276-405, 230-274, 174-228 -- organised around what k_scan_ws's profile showed: it was
 // instruction-issue bound with a share of the issue slots empty, because the four warps of a CTA staged, met at a block barrier, reduced and met again, and every tile
 // started with a dependent chain "load row offsets -> load tails -> gather cur[tail]" of three memory latencies.  Here
 //   * the unit of work is a GROUP of 32 consecutive vertices owned by ONE warp; warps never meet at a block barrier
@@ -94,8 +95,6 @@ k_scan_pw(const ScanParams p, int ngroups, const uint8_t *movable) {
   double *s_wt = reinterpret_cast<double *>(wbase + 2 * CAP * 4);
   uint32_t *s_rows = reinterpret_cast<uint32_t *>(wbase + 2 * CAP * (UNIT ? 4 : 12));
   const uint32_t bar0 = smem_u32(wbase + 2 * CAP * (UNIT ? 4 : 12) + 3 * kPwRows * 4);   // [0,1] tails, [2,3,4] rows
-  __shared__ unsigned long long s_red[3][kPwWarps];
-  __shared__ double s_redd[kPwWarps];
 
   if (lane == 0) {
 #pragma unroll
@@ -238,17 +237,7 @@ k_scan_pw(const ScanParams p, int ngroups, const uint8_t *movable) {
       int cc = 0, best = 0;
       if (mine) { cc = __ldg(p.cur + v); best = cc; }
       double cc_deg = 0.0, vdeg = 0.0, sl = 0.0;
-      if (d && !FIRST) {
-        if (UNIT) {
-          cc_deg = (double)__ldg(at_cdeg<MULTI>(p, cc));
-          vdeg = (double)d;
-          sl = p.has_self ? (double)__ldg(p.self_i + v) : 0.0;
-        } else {
-          cc_deg = __ldg(&at_cinfo_w<MULTI>(p, cc)->degree);
-          vdeg = __ldg(p.vdeg + v);
-          sl = p.has_self ? __ldg(p.self_d + v) : 0.0;
-        }
-      }
+      if (d && !FIRST) vertex_load<UNIT, MULTI>(p, v, cc, d, cc_deg, vdeg, sl);
       __syncwarp();
 
       int lbest = kNoLabel;
@@ -281,83 +270,18 @@ k_scan_pw(const ScanParams p, int ngroups, const uint8_t *movable) {
           }
         }
       } else {
-      // ---- phase B, pass 0: weight towards the own community (counter[0], dspl.hpp:312-318), in edge order; the
-      // other neighbours are compacted to the front of the segment (stable)
-      double w0 = 0.0;
-      int cnt0 = 0, m = 0;
-      for (int k = 0; k < d; k++) {
-        const int x = sc[o0 + k];
-        if (x == cc) { if (UNIT) cnt0++; else w0 += sw[o0 + k]; }
-        else {
-          sc[o0 + m] = x;
-          if (!UNIT) sw[o0 + m] = sw[o0 + k];
-          m++;
-        }
-      }
-      if (UNIT) w0 = (double)cnt0;
-      const double eix = __dsub_rn(w0, sl), ax = __dsub_rn(cc_deg, vdeg);
-      if (d) { if (UNIT) acc_le_u += (unsigned long long)cnt0; else acc_le_d += w0; }
-      if (MASKED && d && !movable[v]) m = 0;                                 // frozen: no candidate, best stays cc
-      // ---- pass 1: two distinct neighbour communities per lane per round (see k_scan_ws)
-      double bg = 0.0;
-      for (;;) {
-        const bool has = m > 0;
-        if (!__any_sync(0xffffffffu, has)) break;
-        int ck1 = 0;
-        double ay1 = 0.0;
-        if (has) {
-          ck1 = sc[o0];
-          if (UNIT) ay1 = (double)__ldg(at_cdeg<MULTI>(p, ck1));
-          else ay1 = __ldg(&at_cinfo_w<MULTI>(p, ck1)->degree);
-        }
-        int ck2 = -1, c1 = 0, c2 = 0, m2 = 0;
-        double sum1 = 0.0, sum2 = 0.0;
-        for (int j = 0; j < m; j++) {
-          const int x = sc[o0 + j];
-          if (x == ck1) { if (UNIT) c1++; else sum1 += sw[o0 + j]; }
-          else {
-            if (ck2 < 0) ck2 = x;
-            if (x == ck2) { if (UNIT) c2++; else sum2 += sw[o0 + j]; }
-            else {
-              sc[o0 + m2] = x;
-              if (!UNIT) sw[o0 + m2] = sw[o0 + j];
-              m2++;
-            }
-          }
-        }
-        m = m2;
-        if (has) {
-          if (UNIT) sum1 = (double)c1;
-          const double g1 = gain_of(sum1, eix, vdeg, ay1, ax, p.constant, p.f32);
-          if (better_l<MULTI>(p, g1, ck1, bg, best, lbest)) { bg = g1; best = ck1; }
-          if (ck2 >= 0) {
-            double ay2;
-            if (UNIT) { ay2 = (double)__ldg(at_cdeg<MULTI>(p, ck2)); sum2 = (double)c2; }
-            else ay2 = __ldg(&at_cinfo_w<MULTI>(p, ck2)->degree);
-            const double g2 = gain_of(sum2, eix, vdeg, ay2, ax, p.constant, p.f32);
-            if (better_l<MULTI>(p, g2, ck2, bg, best, lbest)) { bg = g2; best = ck2; }
-          }
-        }
-      }
-      if (mine && d && label_greater<MULTI>(p, best, lbest, cc)) {             // singleton veto, dspl.hpp:224-225
-        long long sz_cc, sz_b;
-        if (UNIT) {
-          sz_cc = __ldg(at_csize<MULTI>(p, cc));
-          sz_b = __ldg(at_csize<MULTI>(p, best));
-        } else {
-          sz_cc = __ldg(&at_cinfo_w<MULTI>(p, cc)->size);
-          sz_b = __ldg(&at_cinfo_w<MULTI>(p, best)->size);
-        }
-        if (sz_cc == 1 && sz_b == 1) best = cc;
-      }
+        // ---- phase B: the shared per-vertex decision (kernels.cuh)
+        double w0;
+        int m = pass0<UNIT>(sc + o0, sw + o0, d, cc, w0);
+        const double eix = __dsub_rn(w0, sl), ax = __dsub_rn(cc_deg, vdeg);
+        if (d) { if (UNIT) acc_le_u += (unsigned long long)(d - m); else acc_le_d += w0; }
+        if (MASKED && d && !movable[v]) m = 0;                               // frozen: no candidate, best stays cc
+        pass1<UNIT, MULTI>(p, sc + o0, sw + o0, m, eix, vdeg, ax, best, lbest);
+        if (mine) best = singleton_veto<UNIT, MULTI>(p, cc, best, lbest, d);
       }
       if (mine) {
-        if (best != cc) {                                                      // dspl.hpp:331-399
-          if (UNIT) push_move_unit<MULTI>(p, cc, best, d);
-          else push_move_w<MULTI>(p, cc, best, vdeg);
-        }
         p.tgt[v] = best;                                                       // dspl.hpp:404
-        if (TRACE) { acc_moved += (best != cc); acc_hash += vhash(label_of<MULTI>(p, (int)(p.base + v)), label_of<MULTI>(p, best)); }
+        commit<UNIT, MULTI, TRACE>(p, v, cc, best, d, vdeg, acc_moved, acc_hash);
       }
       start = end;
       fence_proxy_async_smem();                  // this lane's generic-proxy accesses to the buffer are ordered before
@@ -369,30 +293,7 @@ k_scan_pw(const ScanParams p, int ngroups, const uint8_t *movable) {
     have_lo = nx_lo; have_n = nx_n;
   }
 
-  if (UNIT) { const unsigned long long s = warp_sum(acc_le_u); if (lane == 0) s_red[0][wid] = s; }
-  else { const double s = warp_sum(acc_le_d); if (lane == 0) s_redd[wid] = s; }
-  if (TRACE) {
-    const unsigned long long a = warp_sum(acc_moved), b = warp_sum(acc_hash);
-    if (lane == 0) { s_red[1][wid] = a; s_red[2][wid] = b; }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (UNIT) {
-      unsigned long long s = 0;
-      for (int w = 0; w < kPwWarps; w++) s += s_red[0][w];
-      if (s) atomicAdd(&p.acc->le_u, s);
-    } else {
-      double s = 0;
-      for (int w = 0; w < kPwWarps; w++) s += s_redd[w];
-      if (s != 0.0) atomicAdd(&p.acc->le_d, s);
-    }
-    if (TRACE) {
-      unsigned long long a = 0, b = 0;
-      for (int w = 0; w < kPwWarps; w++) { a += s_red[1][w]; b += s_red[2][w]; }
-      atomicAdd(&p.acc->moved, a);
-      atomicAdd(&p.acc->hash, b);
-    }
-  }
+  flush_acc<UNIT, TRACE, kPwWarps>(p, acc_le_u, acc_le_d, acc_moved, acc_hash);
 }
 
 }  // namespace mv

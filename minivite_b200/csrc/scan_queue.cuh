@@ -55,7 +55,6 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
   int32_t *q_ent = reinterpret_cast<int32_t *>(wbase + CAP * 4 + 3 * kPwRows * 4);
   int4 *q_hdr = reinterpret_cast<int4 *>(wbase + CAP * 4 + 3 * kPwRows * 4 + kQSlots * kQEnt * 4);
   const uint32_t bar0 = smem_u32(wbase + CAP * 4 + 3 * kPwRows * 4 + kQSlots * kQEnt * 4 + kQSlots * 16);   // [0] tails, [1..3] rows
-  __shared__ unsigned long long s_red[3][kPwWarps];
 
   if (lane == 0) {
 #pragma unroll
@@ -92,50 +91,19 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
     lo4 = e0 & ~3u;
     n4 = (e1 > lo4) ? min((uint32_t)CAP, (e1 - lo4 + 3u) & ~3u) : 0u;
   };
-  // pass 1 + decision for one vertex whose leftover communities sit in seg[0..m): two communities per round, exactly
-  // k_scan_pw's loop.  Lanes without work pass m = 0.  Returns the chosen community.
+  // pass 1 + singleton veto (kernels.cuh) for one vertex whose leftover communities sit in seg[0..m).  All lanes call
+  // it; lanes without work pass m = 0.  Returns the chosen community.
   // (The same bound per candidate -- skip the exact gain when fl(2 (c - e_ix) + gB) is below the best gain so far -- was
   // measured and removed: the test costs more double-precision instructions than it saves, scan 15.30 -> 15.68 ms.)
-  auto pass1 = [&](int32_t *seg, int m, int cc, double eix, double vdeg, double ax) -> int {
+  auto decide = [&](int32_t *seg, int m, int cc, int d, double eix, double vdeg, double ax) -> int {
     int best = cc, lbest = kNoLabel;
-    double bg = 0.0;
-    for (;;) {
-      const bool has = m > 0;
-      if (!__any_sync(0xffffffffu, has)) break;
-      int ck1 = 0;
-      double ay1 = 0.0;
-      if (has) { ck1 = seg[0]; ay1 = (double)__ldg(at_cdeg<MULTI>(p, ck1)); }
-      int ck2 = -1, c1 = 0, c2 = 0, m2 = 0;
-      for (int j = 0; j < m; j++) {
-        const int x = seg[j];
-        if (x == ck1) c1++;
-        else {
-          if (ck2 < 0) ck2 = x;
-          if (x == ck2) c2++;
-          else { seg[m2] = x; m2++; }
-        }
-      }
-      m = m2;
-      if (has) {
-        const double g1 = gain_of((double)c1, eix, vdeg, ay1, ax, p.constant, p.f32);
-        if (better_l<MULTI>(p, g1, ck1, bg, best, lbest)) { bg = g1; best = ck1; }
-        if (ck2 >= 0) {
-          const double ay2 = (double)__ldg(at_cdeg<MULTI>(p, ck2));
-          const double g2 = gain_of((double)c2, eix, vdeg, ay2, ax, p.constant, p.f32);
-          if (better_l<MULTI>(p, g2, ck2, bg, best, lbest)) { bg = g2; best = ck2; }
-        }
-      }
-    }
-    if (best != cc && label_greater<MULTI>(p, best, lbest, cc)) {               // singleton veto, dspl.hpp:224-225
-      if (__ldg(at_csize<MULTI>(p, cc)) == 1 && __ldg(at_csize<MULTI>(p, best)) == 1) best = cc;
-    }
-    return best;
+    pass1<true, MULTI>(p, seg, nullptr, m, eix, vdeg, ax, best, lbest);
+    return singleton_veto<true, MULTI>(p, cc, best, lbest, d);
   };
   // targetComm, deltas, trace for one vertex (dspl.hpp:331-404)
   auto finish = [&](int v, int cc, int best, int d) {
-    if (best != cc) push_move_unit<MULTI>(p, cc, best, d);
     p.tgt[v] = best;
-    if (TRACE) { acc_moved += (best != cc); acc_hash += vhash(label_of<MULTI>(p, (int)(p.base + v)), label_of<MULTI>(p, best)); }
+    commit<true, MULTI, TRACE>(p, v, cc, best, d, 0.0, acc_moved, acc_hash);
   };
   // run pass 1 for up to 32 parked vertices, one per lane
   auto drain = [&](int n) {
@@ -146,7 +114,7 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
     const int m = on ? (h.z & 0xffff) : 0, d = h.z >> 16;
     const double vdeg = (double)d, sl = (on && p.has_self) ? (double)__ldg(p.self_i + h.x) : 0.0;
     const double eix = __dsub_rn((double)(d - m), sl), ax = __dsub_rn((double)(unsigned int)h.w, vdeg);
-    const int best = pass1(q_ent + slot * kQEnt, m, h.y, eix, vdeg, ax);
+    const int best = decide(q_ent + slot * kQEnt, m, h.y, d, eix, vdeg, ax);
     if (on) finish(h.x, h.y, best, d);
     qhead = (qhead + n) % kQSlots;
     qcount -= n;
@@ -242,16 +210,13 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
       }
       __syncwarp();
 
-      // ---- pass 0 (counter[0], dspl.hpp:312-318): count the own community, compact the others to the front
+      // ---- pass 0 (kernels.cuh): count the own community, compact the others to the front
       int32_t *const seg = sc + o0;
-      int m = 0;
-      for (int k = 0; k < d; k++) {
-        const int x = seg[k];
-        if (x != cc) { seg[m] = x; m++; }
-      }
+      double w0;
+      const int m = pass0<true>(seg, nullptr, d, cc, w0);
       if (d) acc_le_u += (unsigned long long)(d - m);
       const double vdeg = (double)d;
-      const double eix = __dsub_rn((double)(d - m), sl), ax = __dsub_rn((double)cc_deg_u, vdeg);
+      const double eix = __dsub_rn(w0, sl), ax = __dsub_rn((double)cc_deg_u, vdeg);
       // ---- can any candidate beat maxGain = 0?  (see the header: exact upper bound on curGain)
       const double gB = __dmul_rn(__dmul_rn(__dmul_rn(2.0, vdeg), ax), p.constant);
       const double bound = __dadd_rn(__dmul_rn(2.0, __dsub_rn((double)m, eix)), gB);
@@ -261,7 +226,7 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
       const bool in_place = __any_sync(0xffffffffu, hard && m > kQEnt);
       if (in_place) {
         // early iterations: long leftover lists everywhere -> pass 1 where the lists are, like k_scan_pw
-        const int best = pass1(seg, hard ? m : 0, cc, eix, vdeg, ax);
+        const int best = decide(seg, hard ? m : 0, cc, d, eix, vdeg, ax);
         if (mine) finish(v, cc, best, d);
       } else {
         if (mine && !hard) finish(v, cc, cc, d);
@@ -293,23 +258,7 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
   }
   while (qcount > 0) drain(min(qcount, 32));
 
-  { const unsigned long long s = warp_sum(acc_le_u); if (lane == 0) s_red[0][wid] = s; }
-  if (TRACE) {
-    const unsigned long long a = warp_sum(acc_moved), b = warp_sum(acc_hash);
-    if (lane == 0) { s_red[1][wid] = a; s_red[2][wid] = b; }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long s = 0;
-    for (int w = 0; w < kPwWarps; w++) s += s_red[0][w];
-    if (s) atomicAdd(&p.acc->le_u, s);
-    if (TRACE) {
-      unsigned long long a = 0, b = 0;
-      for (int w = 0; w < kPwWarps; w++) { a += s_red[1][w]; b += s_red[2][w]; }
-      atomicAdd(&p.acc->moved, a);
-      atomicAdd(&p.acc->hash, b);
-    }
-  }
+  flush_acc<true, TRACE, kPwWarps>(p, acc_le_u, 0.0, acc_moved, acc_hash);
 }
 
 }  // namespace mv
