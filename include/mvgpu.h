@@ -240,6 +240,37 @@ int mvgpu_compare_communities(mvgpu_ctx *ctx, const int64_t *x, const int64_t *y
  * failed one, and after the next upload, attach or generate.  Any of the four arrays may be NULL (not written). */
 int mvgpu_get_community_matches(mvgpu_ctx *ctx, int64_t *size, int64_t *best, int64_t *overlap, int64_t *best_size);
 
+/* ---- probing an assignment (DESIGN.md §3.15) ------------------------------------------------------------------------
+ * What every vertex would do under the Louvain rule from assignment X, with the quantities iteration 1 of a warm run from
+ * X reads: counter[0], the self-loop weight, vDegree, a_x / size_x and a_y / size_y of every community under X over all
+ * ranks, and c = 1/(2m) as a run computes it.  For vertex i with x = X(i):
+ *   candidates  the communities y != x of the tails of i's records;
+ *   gain(i, y)  dspl.hpp:212 with the reference's association (2.0*(e_iy - e_ix) - ((2.0*k_i)*(a_y - a_x))*c);
+ *   best(i)     the candidate with the largest gain, equal gains to the smallest id; -1 without a candidate (no records,
+ *               only self loops, or every neighbour in x);
+ *   gain(i)     gain(i, best(i)), which may be negative or zero; -inf when best = -1 (the stability margin);
+ *   target(i)   the reference's decision (dspl.hpp:174-228, 309-324): best(i) if gain(i) > 0 and the singleton veto
+ *               (size_x = size_best = 1 and best > x) does not fire, else x.
+ * A movable set does not restrict the probe: it says what each vertex would do if it were movable.  Unit and dyadic
+ * weights give the same bits on every rank count and every option (reorder, force_heavy_deg, force_weighted, upload mode). */
+typedef struct {
+  int64_t vertices;   /* nv */
+  int64_t moves;      /* #{i : target(i) != X(i)}: 0 iff X is a fixed point of the rule */
+  int64_t vetoed;     /* #{i : gain(i) > 0, kept in place by the singleton veto} */
+  int64_t interior;   /* #{i : i has records and best(i) = -1} */
+  double max_gain;    /* max over i of gain(i); -inf when no vertex has a candidate */
+  double constant;    /* c = 1/(2m) used */
+  double probe_s;     /* device time of the call (CUDA events on the context's stream) */
+} mvgpu_probe_report;
+/* Collective.  comm: lnv community ids in [0, nv) in the caller's vertex numbering (the form mvgpu_evaluate_communities
+ * takes); NULL probes the assignment the last mvgpu_louvain on this shard returned.  target, best (caller ids) and gain
+ * hold lnv entries each; any of them may be NULL (not written).  Errors as in mvgpu_evaluate_communities (a bad id on any
+ * rank, NULL without a run, ranks that disagree on NULL, a shard from mvgpu_upload_shard32) fail the call on every rank,
+ * and then nothing is written.  Changes nothing else: everything the last run reports, the initial assignment, the
+ * movable set and the arrays of the last evaluation and the last comparison stay as they were. */
+int mvgpu_probe_communities(mvgpu_ctx *ctx, const int64_t *comm, int64_t *target, int64_t *best, double *gain,
+                            mvgpu_probe_report *rep);
+
 /* currComm of this rank's vertices at exit (global community ids), lnv entries, of the last mvgpu_louvain on the current
  * shard: it fails with "no run on this shard" after an upload / attach / generate until the new shard's first run;
  * mvgpu_update_shard keeps serving the last run's result. */

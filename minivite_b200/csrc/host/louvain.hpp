@@ -36,6 +36,9 @@ struct GpuRankContext {
   const std::vector<unsigned char> *movable = nullptr; // -V: movable set of this rank's vertices (nonzero = movable)
   bool frontier = false;                               // -F: grow the movable set from the vertices that move
   std::vector<unsigned char> *movable_out = nullptr;   // -o: the set the next iteration would use (for -V on resume)
+  bool probe = false;                                  // -U: probe the assignment -q would evaluate
+  mvgpu_probe_report probe_rep{};                      // -U: the probe's counts (global values)
+  std::vector<unsigned char> unsettled;                // -U with -o: 1 where the probe's target differs from the assignment
 };
 
 [[noreturn]] inline void mv_abort(const std::string &where) {
@@ -89,6 +92,21 @@ inline void mv_compare(mvgpu_ctx *ctx, GpuRankContext &rc, const GraphElem *X) {
   const GraphElem *Y = rc.cmp_comm->empty() ? &none : rc.cmp_comm->data();
   if (mvgpu_compare_communities(ctx, X, Y, &rc.cmp)) mv_abort("mvgpu_compare_communities");
 }
+// -U: probe X (NULL: the run's result); with -o, mark the vertices whose target is not their community
+inline void mv_probe(mvgpu_ctx *ctx, GpuRankContext &rc, const GraphElem *X, GraphElem lnv) {
+  if (!rc.probe) return;
+  std::vector<int64_t> target(lnv + 1);            // never an empty array
+  if (mvgpu_probe_communities(ctx, X, target.data(), nullptr, nullptr, &rc.probe_rep)) mv_abort("mvgpu_probe_communities");
+  if (!rc.comm_out) return;
+  std::vector<int64_t> run;
+  if (!X) {
+    run.resize(lnv + 1);
+    if (lnv && mvgpu_get_communities(ctx, run.data())) mv_abort("mvgpu_get_communities");
+    X = run.data();
+  }
+  rc.unsettled.resize(lnv);
+  for (GraphElem i = 0; i < lnv; i++) rc.unsettled[i] = target[i] != X[i] ? 1 : 0;
+}
 // -E: evaluate the given assignment (with -C: its split) and run no Louvain phase (true: done, the caller returns)
 inline bool mv_evaluate_only(mvgpu_ctx *ctx, GpuRankContext &rc) {
   if (!rc.eval_comm) return false;
@@ -98,14 +116,17 @@ inline bool mv_evaluate_only(mvgpu_ctx *ctx, GpuRankContext &rc) {
     X = rc.split_comm.data();
   }
   mv_compare(ctx, rc, X);
+  mv_probe(ctx, rc, X, (GraphElem)rc.eval_comm->size());
   if (mvgpu_evaluate_communities(ctx, X, &rc.q)) mv_abort("mvgpu_evaluate_communities");
   mvgpu_destroy(ctx);
   return true;
 }
-// -C: split the assignment the run returned; -M: compare the run's assignment (with -C: its split); -q: evaluate it
+// -C: split the assignment the run returned; -M: compare the run's assignment (with -C: its split); -U: probe it; -q:
+// evaluate it
 inline void mv_evaluate_run(mvgpu_ctx *ctx, GpuRankContext &rc, GraphElem lnv) {
   if (rc.split) mv_split(ctx, rc, nullptr, lnv);
   mv_compare(ctx, rc, rc.split ? rc.split_comm.data() : nullptr);
+  mv_probe(ctx, rc, rc.split ? rc.split_comm.data() : nullptr, lnv);
   if (rc.quality && mvgpu_evaluate_communities(ctx, rc.split ? rc.split_comm.data() : nullptr, &rc.q))
     mv_abort("mvgpu_evaluate_communities");
 }

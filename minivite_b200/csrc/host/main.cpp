@@ -16,6 +16,9 @@
 //            writes the split assignment (prints SPLIT communities=.. components=.. disconnected=.. rounds=..)
 //            -M <prefix> compare the assignment -q would evaluate with the communities an earlier -o <prefix> wrote
 //            (prints COMPARE ari=.. nmi=.. vi=.. rand=.. mi=.. hx=.. hy=.. cells=.. communities_x=.. communities_y=..)
+//            -U probe the assignment -q would evaluate: what every vertex would do under the Louvain rule from it (prints
+//            PROBE vertices=.. moves=.. vetoed=.. interior=.. max_gain=..); with -o also <o>.unsettled.<rank>, lnv bytes,
+//            1 where the vertex would move, in the -V format: -i <o> -V <o>.unsettled -F re-clusters from those vertices
 #include <getopt.h>
 #include <sys/mman.h>
 #include <sys/wait.h>
@@ -43,7 +46,7 @@ static int me = 0, nprocs = 1;
 static int ranksPerNode = 1;
 static GraphElem nvRGG = 0;
 static bool generateGraph = false, readBalanced = false, showGraph = false, traceIters = false, deviceGenerate = false,
-            evalQuality = false, splitComm = false;
+            evalQuality = false, splitComm = false, probeComm = false;
 static GraphWeight randomEdgePercent = 0.0;
 static bool randomNumberLCG = false, isUnitEdgeWeight = true;
 static GraphWeight threshold = 1.0E-6;
@@ -92,7 +95,7 @@ static long long reduce_sum_ll(long long v) {
 
 static void parseCommandLine(const int argc, char *const argv[]) {
   int ret;
-  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:CM:V:F")) != -1) {
+  while ((ret = getopt(argc, argv, "f:br:t:n:wlp:sg:o:TDi:k:L:qE:CM:V:FU")) != -1) {
     switch (ret) {
       case 'f': inputFileName.assign(optarg); break;
       case 'b': readBalanced = true; break;
@@ -116,6 +119,7 @@ static void parseCommandLine(const int argc, char *const argv[]) {
       case 'M': comparePrefix.assign(optarg); break;
       case 'V': movablePrefix.assign(optarg); break;
       case 'F': frontierGrow = true; break;
+      case 'U': probeComm = true; break;
       default: assert(0 && "Option not recognized!!!"); break;
     }
   }
@@ -296,6 +300,7 @@ int main(int argc, char *argv[]) {
   rc.stop_after = stopAfter;
   rc.quality = evalQuality;
   rc.split = splitComm;
+  rc.probe = probeComm;
 
   GraphWeight currMod = lowerStart;
   std::vector<GraphElem> ssizes, rsizes, svdata, rvdata;
@@ -334,6 +339,9 @@ int main(int argc, char *argv[]) {
     fprintf(stderr, "COMPARE ari=%.17g nmi=%.17g vi=%.17g rand=%.17g mi=%.17g hx=%.17g hy=%.17g cells=%ld communities_x=%ld "
             "communities_y=%ld\n", rc.cmp.ari, rc.cmp.nmi, rc.cmp.vi, rc.cmp.rand, rc.cmp.mi, rc.cmp.h_x, rc.cmp.h_y,
             (long)rc.cmp.cells, (long)rc.cmp.communities_x, (long)rc.cmp.communities_y);
+  if (me == 0 && probeComm)
+    fprintf(stderr, "PROBE vertices=%ld moves=%ld vetoed=%ld interior=%ld max_gain=%.17g\n", (long)rc.probe_rep.vertices,
+            (long)rc.probe_rep.moves, (long)rc.probe_rep.vetoed, (long)rc.probe_rep.interior, rc.probe_rep.max_gain);
   if (me == 0 && (evalQuality || !evalPrefix.empty()))
     fprintf(stderr, "QUALITY mod=%.17g e=%.17g a2=%.17g communities=%ld singletons=%ld maxsize=%ld\n", rc.q.modularity,
             rc.q.e_in, rc.q.a2, (long)rc.q.communities, (long)rc.q.singletons, (long)rc.q.max_size);
@@ -352,6 +360,11 @@ int main(int argc, char *argv[]) {
     FILE *fm = fopen((dumpPrefix + ".mask." + std::to_string(me)).c_str(), "wb");
     fwrite(movableOut.data(), 1, movableOut.size(), fm);
     fclose(fm);
+    if (probeComm) {
+      FILE *fu = fopen((dumpPrefix + ".unsettled." + std::to_string(me)).c_str(), "wb");
+      fwrite(rc.unsettled.data(), 1, rc.unsettled.size(), fu);
+      fclose(fu);
+    }
   }
   if (me == 0 && evalPrefix.empty()) {            // (-E ran no Louvain phase: nothing to report)
     const double avgt = tot_time / nprocs, avgd = dev_time / nprocs;

@@ -216,11 +216,12 @@ __device__ __forceinline__ int label_of(const ScanParams &p, int c) {
   if (!p.relabel) return c;
   return __ldg(at_lab<MULTI>(p, c));
 }
-// better() with lazily fetched labels; lby caches the label of the current best (kNoLabel = not fetched)
-template <bool MULTI>
+// better() with lazily fetched labels; lby caches the label of the current best (kNoLabel = not fetched).
+// ANY_TIE: equal gains of any value, zero included, go to the smaller label (the probe's best candidate, probe_gpu.cuh)
+template <bool MULTI, bool ANY_TIE = false>
 __device__ __forceinline__ bool better_l(const ScanParams &p, double g, int y, double bg, int by, int &lby) {
   if (g > bg) { lby = kNoLabel; return true; }
-  if ((g == bg) && (g != 0.0)) {
+  if ((g == bg) && (ANY_TIE || g != 0.0)) {
     const int ly = label_of<MULTI>(p, y);
     if (lby == kNoLabel) lby = label_of<MULTI>(p, by);
     if (ly < lby) { lby = ly; return true; }
@@ -307,10 +308,13 @@ __device__ __forceinline__ int pass0(int32_t *seg, double *segw, int d, int cc, 
 // community degree gather issued before the walk is consumed after it.  best/lbest come in as the current community /
 // kNoLabel and leave as the winner under dspl.hpp:214-215 and its cached label.
 // All 32 lanes of the warp must call it (__any_sync); a lane without work passes m = 0.
-template <bool UNIT, bool MULTI>
+// MARGIN (mvgpu_probe_communities, probe_gpu.cuh): the walk starts at -inf instead of 0 and equal gains of any value go
+// to the smaller label, so best (coming in as -1) leaves as the best candidate whatever its gain, and *margin receives
+// that gain (-inf: no candidate).
+template <bool UNIT, bool MULTI, bool MARGIN = false>
 __device__ __forceinline__ void pass1(const ScanParams &p, int32_t *seg, double *segw, int m, double eix, double vdeg,
-                                      double ax, int &best, int &lbest) {
-  double bg = 0.0;
+                                      double ax, int &best, int &lbest, double *margin = nullptr) {
+  double bg = MARGIN ? -INFINITY : 0.0;
   for (;;) {
     const bool has = m > 0;
     if (!__any_sync(0xffffffffu, has)) break;
@@ -340,16 +344,17 @@ __device__ __forceinline__ void pass1(const ScanParams &p, int32_t *seg, double 
     if (has) {
       if (UNIT) sum1 = (double)c1;
       const double g1 = gain_of(sum1, eix, vdeg, ay1, ax, p.constant, p.f32);
-      if (better_l<MULTI>(p, g1, ck1, bg, best, lbest)) { bg = g1; best = ck1; }
+      if (better_l<MULTI, MARGIN>(p, g1, ck1, bg, best, lbest)) { bg = g1; best = ck1; }
       if (ck2 >= 0) {
         double ay2;
         if (UNIT) { ay2 = (double)__ldg(at_cdeg<MULTI>(p, ck2)); sum2 = (double)c2; }
         else ay2 = __ldg(&at_cinfo_w<MULTI>(p, ck2)->degree);
         const double g2 = gain_of(sum2, eix, vdeg, ay2, ax, p.constant, p.f32);
-        if (better_l<MULTI>(p, g2, ck2, bg, best, lbest)) { bg = g2; best = ck2; }
+        if (better_l<MULTI, MARGIN>(p, g2, ck2, bg, best, lbest)) { bg = g2; best = ck2; }
       }
     }
   }
+  if (MARGIN) *margin = bg;
 }
 
 // singleton veto (dspl.hpp:224-225) for vertex of degree d: a singleton does not move to a singleton of larger label.

@@ -37,6 +37,7 @@
 #include "rgg_gpu.cuh"
 #include "merge_gpu.cuh"
 #include "compare_gpu.cuh"
+#include "probe_gpu.cuh"
 
 // host-only helper of the compact upload (narrow.cpp): 16-byte edge records -> 4-byte tails + validation
 extern "C" void mv_narrow_edges(const void *edge_records, long long n, long long nv, long long base, long long bound,
@@ -259,6 +260,9 @@ struct mvgpu_ctx {
   DevBuf<CmpRow> cmp_row0, cmp_row1;
   DevBuf<long long> cmp_match, cmp_off;
   DevBuf<int> cmp_n;
+  // probing (mvgpu_probe_communities): target, best (int32 caller ids) and gain per own vertex; nothing is peer-exported
+  DevBuf<int32_t> probe_tgt, probe_best;
+  DevBuf<double> probe_gain;
   bool run_on_shard = false;           // final_orig holds a run's assignment of the current shard
   bool eval_on_shard = false;          // the q_* arrays describe an evaluation of the current shard
   bool cmp_on_shard = false;           // cmp_match describes a successful comparison on the current shard's vertices
@@ -315,6 +319,7 @@ struct Scalars {
   unsigned long long span_sum, span_cnt;
   unsigned long long q_agg[2];         // evaluation: singletons, largest community
   unsigned long long split_agg[3];     // splitting: non-empty communities, components, disconnected communities
+  unsigned long long probe_agg[4];     // probing: moves, vetoed, interior, largest gain as probe_key (ProbeOut::agg)
 };
 Scalars *dev_scalars(mvgpu_ctx *c) { return reinterpret_cast<Scalars *>(c->scratch.p); }
 
@@ -641,6 +646,7 @@ struct EvalSetup {
   const int32_t *X = nullptr;
   bool given = false;                  // the caller passed an array (not NULL)
   bool split = false;                  // for mvgpu_split_communities: the labels are allocated and exported too
+  bool probe = false;                  // for mvgpu_probe_communities: the evaluation's arrays are left alone
   std::string err;
 };
 
@@ -703,7 +709,7 @@ int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, 
     // CUDA IPC requires every peer to close its mapping before the owner frees the block, so growing an exported array
     // is agreed on here and done collectively (need_s: init_state's bound lnv + #non-owned edge tails >= lnv + nghost)
     Export x[kPeerArrays];
-    exports(c, x, (size_t)c->lnv, (size_t)(c->lnv + nremote), ev != nullptr, ev && ev->split);
+    exports(c, x, (size_t)c->lnv, (size_t)(c->lnv + nremote), ev && !ev->probe, ev && ev->split);
     bool grow = false;
     for (const Export &e : x) grow = grow || (c->ipc_valid && e.cap && e.cap < e.need);
     const bool assigned = ev ? ev->given : c->warm_run;
@@ -718,8 +724,8 @@ int setup_agree(mvgpu_ctx *c, const EvalSetup *ev, long long nremote, int unit, 
     if (err.empty() && !partition_agrees(c, hv + 7)) err = kPartitionDisagree;
     if (hv[2] && err.empty()) err = ev ? "another rank rejected its shard or its assignment" : "another rank rejected its shard";
     if (err.empty() && hv[4] != 0 && hv[4] != c->nranks)
-      err = ev ? (ev->split ? "ranks disagree on the assignment to split: every rank or none must pass NULL"
-                            : "ranks disagree on the assignment to evaluate: every rank or none must pass NULL")
+      err = ev ? std::string("ranks disagree on the assignment to ") + (ev->split ? "split" : ev->probe ? "probe" : "evaluate") +
+                     ": every rank or none must pass NULL"
                : "ranks disagree on the initial assignment: every rank or none must set one";
     if (err.empty() && hv[5] != 0 && hv[5] != c->nranks)
       err = "ranks disagree on the movable set: every rank or none must set one (mvgpu_set_movable)";
@@ -947,7 +953,7 @@ int init_state(mvgpu_ctx *c, const EvalSetup *ev, long long nremote) {
   else { TRY(c->cinfo_w.ensure(lnv)); TRY(c->usize.ensure(lnv)); TRY(c->udeg.ensure(lnv)); TRY(c->vdeg.ensure(lnv)); TRY(c->self_d.ensure(lnv)); }
   TRY(c->acc.ensure((size_t)c->opt_max_iters + 2));
   CK(cudaMemsetAsync(c->acc.p, 0, sizeof(Acc) * ((size_t)c->opt_max_iters + 2), s));
-  if (ev) {                                   // zeroed before warm_init's last barrier: no peer adds to it earlier
+  if (ev && !ev->probe) {                     // zeroed before warm_init's last barrier: no peer adds to it earlier
     TRY(c->q_internal.ensure(lnv)); TRY(c->q_rank.ensure(lnv + 1));
     CK(cudaMemsetAsync(c->q_internal.p, 0, sizeof(double) * lnv, s));
     if (ev->split) TRY(c->split_lab.ensure(lnv));
@@ -1138,6 +1144,22 @@ double modularity(double e, double a2, double cst) {
   return term1 - term2;
 }
 
+// what the scan kernels read of the state setup_run left (cur, tgt and acc are per iteration: the caller's)
+ScanParams scan_params(const mvgpu_ctx *c) {
+  ScanParams sp;
+  memset(&sp, 0, sizeof sp);
+  sp.lnv = (int)c->lnv; sp.has_self = c->scan_has_self; sp.heavy_deg = c->scan_heavy_deg; sp.has_heavy = c->nheavy > 0; sp.base = c->base;
+  sp.cache_policy = c->opt_cache_policy;
+  sp.relabel = c->relabel;
+  sp.rowptr = c->a_rowptr; sp.tails = c->a_tails; sp.weights = c->unit ? nullptr : c->a_weights;
+  sp.self_i = c->self_i.p; sp.self_d = c->self_d.p; sp.vdeg = c->vdeg.p; sp.constant = c->constant; sp.f32 = c->f32 ? 1 : 0;
+  sp.heavy_list = c->heavy_list.p; sp.heavy_off = c->heavy_off.p; sp.hkeys = c->hkeys.p; sp.hvals_d = c->hvals_d.p; sp.hvals_i = c->hvals_i.p;
+  sp.pt = c->pt;
+  sp.loc_cdeg = c->cdeg.p; sp.loc_csize = c->csize.p; sp.loc_upd = c->upd.p; sp.loc_cinfo_w = c->cinfo_w.p;
+  sp.loc_usize = c->usize.p; sp.loc_udeg = c->udeg.p; sp.loc_lab = c->relabel ? c->lab.p : nullptr;
+  return sp;
+}
+
 int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, double *mod_out) {
   TRY(check_ready(c));
   CK(cudaSetDevice(c->device));
@@ -1153,17 +1175,7 @@ int run_louvain(mvgpu_ctx *c, double lower, double thresh, int *iters_out, doubl
   CK(cudaEventRecord(e_setup, s));
 
   int32_t *cur = c->comm_a.p, *tgt = c->comm_b.p;
-  ScanParams sp;
-  memset(&sp, 0, sizeof sp);
-  sp.lnv = (int)c->lnv; sp.has_self = c->scan_has_self; sp.heavy_deg = c->scan_heavy_deg; sp.has_heavy = c->nheavy > 0; sp.base = c->base;
-  sp.cache_policy = c->opt_cache_policy;
-  sp.relabel = c->relabel;
-  sp.rowptr = c->a_rowptr; sp.tails = c->a_tails; sp.weights = c->unit ? nullptr : c->a_weights;
-  sp.self_i = c->self_i.p; sp.self_d = c->self_d.p; sp.vdeg = c->vdeg.p; sp.constant = c->constant; sp.f32 = c->f32 ? 1 : 0;
-  sp.heavy_list = c->heavy_list.p; sp.heavy_off = c->heavy_off.p; sp.hkeys = c->hkeys.p; sp.hvals_d = c->hvals_d.p; sp.hvals_i = c->hvals_i.p;
-  sp.pt = c->pt;
-  sp.loc_cdeg = c->cdeg.p; sp.loc_csize = c->csize.p; sp.loc_upd = c->upd.p; sp.loc_cinfo_w = c->cinfo_w.p;
-  sp.loc_usize = c->usize.p; sp.loc_udeg = c->udeg.p; sp.loc_lab = c->relabel ? c->lab.p : nullptr;
+  ScanParams sp = scan_params(c);
   // movable set: M_k in mov[k_cur]; with the frontier option the scan's movers grow M_{k+1} into the other buffer,
   // every rank's (mp[b] addresses buffer b on every rank), and an accepted iteration swaps them like cur / tgt
   uint8_t *mov[2] = {c->mov_a.p, c->mov_b.p};
@@ -1557,6 +1569,85 @@ int split(mvgpu_ctx *c, const int64_t *comm, int64_t *out, mvgpu_split_report *r
     k_widen<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(c->split_lab.p, c->lnv, c->wide.p);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * c->lnv, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+  }
+  *rep = r;
+  return 0;
+}
+
+// ---- probing (DESIGN.md §3.15, probe_gpu.cuh): after setup_run(ev), comm_a = X on every slot and the Comm records are
+// X's, so the scan's per-vertex rule reads exactly what iteration 1 of a warm run from X reads
+template <bool UNIT, bool MULTI>
+int launch_probe_t(mvgpu_ctx *c, const ScanParams &sp, const ProbeOut &o) {
+  const int tiles = (int)((c->lnv + kTileV - 1) / kTileV);
+  if (tiles > 0) {
+    k_probe<UNIT, MULTI><<<tiles, kTileV, UNIT ? sizeof(int32_t) * kECap : (sizeof(int32_t) + sizeof(double)) * kECap, c->stream>>>(sp, o);
+    c->tm.kernel_launches++;
+  }
+  if (c->nheavy > 0) {
+    k_probe_heavy<UNIT, MULTI><<<(int)c->nheavy, 256, 0, c->stream>>>(sp, o);
+    c->tm.kernel_launches++;
+  }
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int probe_pass(mvgpu_ctx *c, mvgpu_probe_report &rep) {
+  cudaStream_t s = c->stream;
+  Scalars *d_sc = dev_scalars(c);               // probe_agg was zeroed with the other scalars at the start of setup_run
+  TRY(c->probe_tgt.ensure(c->lnv)); TRY(c->probe_best.ensure(c->lnv)); TRY(c->probe_gain.ensure(c->lnv));
+  ScanParams sp = scan_params(c);
+  sp.cur = c->comm_a.p;
+  const ProbeOut o = {c->probe_tgt.p, c->probe_best.p, c->probe_gain.p, d_sc->probe_agg};
+  const bool multi = c->nranks > 1;
+  int (*launch)(mvgpu_ctx *, const ScanParams &, const ProbeOut &) =
+      c->unit ? (multi ? launch_probe_t<true, true> : launch_probe_t<true, false>)
+              : (multi ? launch_probe_t<false, true> : launch_probe_t<false, false>);
+  TRY(launch(c, sp, o));
+  unsigned long long agg[4];
+  CK(cudaMemcpyAsync(agg, d_sc->probe_agg, sizeof agg, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  // every rank's kernels have finished (and stopped reading its peers' Comm records) once these collectives return
+  long long n[3] = {(long long)agg[0], (long long)agg[1], (long long)agg[2]};
+  TRY(coll_allreduce_i64(c, n, 3, false));
+  long long kmax = (long long)(agg[3] ^ (1ULL << 63));   // unsigned key order as signed order
+  TRY(coll_allreduce_i64(c, &kmax, 1, true));
+  const unsigned long long key = (unsigned long long)kmax ^ (1ULL << 63);
+  const unsigned long long bits = (key >> 63) ? (key & ~(1ULL << 63)) : ~key;
+  double g;
+  memcpy(&g, &bits, sizeof g);
+  rep.vertices = c->nv_global;
+  rep.moves = n[0]; rep.vetoed = n[1]; rep.interior = n[2];
+  rep.max_gain = key ? g : -INFINITY;
+  rep.constant = c->constant;
+  return 0;
+}
+
+// collective like evaluate; target / best / gain are written only when the call succeeds
+int probe(mvgpu_ctx *c, const int64_t *comm, int64_t *target, int64_t *best, double *gain, mvgpu_probe_report *rep,
+          const char *caller_err = nullptr) {
+  TRY(check_ready(c));
+  CK(cudaSetDevice(c->device));
+  if (c->run_on_shard) TRY(final_in_caller_order(c));   // as in evaluate: setup_run overwrites comm_a
+  EvalSetup ev;
+  ev.probe = true;
+  TRY(take_assignment(c, comm, "mvgpu_probe_communities", "probes", caller_err, ev));
+  mvgpu_probe_report r;
+  memset(&r, 0, sizeof r);
+  TRY(assignment_pass(c, ev, [&] { return probe_pass(c, r); }, r.probe_s));
+  const long long lnv = c->lnv;
+  if (lnv > 0) {
+    int32_t *src[2] = {c->probe_tgt.p, c->probe_best.p};
+    int64_t *dst[2] = {target, best};
+    for (int k = 0; k < 2; k++) {
+      if (!dst[k]) continue;
+      TRY(c->wide.ensure(lnv));
+      k_widen<<<grid_for(lnv, 256, c->num_sms), 256, 0, c->stream>>>(src[k], lnv, c->wide.p);
+      CK(cudaGetLastError());
+      CK(cudaMemcpyAsync(dst[k], c->wide.p, sizeof(long long) * lnv, cudaMemcpyDeviceToHost, c->stream));
+      CK(cudaStreamSynchronize(c->stream));
+    }
+    if (gain) CK(cudaMemcpyAsync(gain, c->probe_gain.p, sizeof(double) * lnv, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
   }
   *rep = r;
@@ -2449,6 +2540,18 @@ int mv_split_refused(mvgpu_ctx *c, const char *why, mvgpu_split_report *rep) {
   if (!c || !rep || !why) return fail("null argument");
   int64_t none = 0;
   return split(c, nullptr, &none, rep, why);
+}
+
+int mvgpu_probe_communities(mvgpu_ctx *c, const int64_t *comm, int64_t *target, int64_t *best, double *gain,
+                            mvgpu_probe_report *rep) {
+  if (!c || !rep) return fail("null argument");
+  return probe(c, comm, target, best, gain, rep);
+}
+
+// Not in mvgpu.h: the Python binding's way into the collective when it cannot build the array, as mv_evaluate_refused
+int mv_probe_refused(mvgpu_ctx *c, const char *why, mvgpu_probe_report *rep) {
+  if (!c || !rep || !why) return fail("null argument");
+  return probe(c, nullptr, nullptr, nullptr, nullptr, rep, why);
 }
 
 int mvgpu_compare_communities(mvgpu_ctx *c, const int64_t *x, const int64_t *y, mvgpu_compare_report *rep) {

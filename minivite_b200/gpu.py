@@ -54,6 +54,15 @@ class CompareReport(ctypes.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class ProbeReport(ctypes.Structure):
+    _fields_ = [("vertices", ctypes.c_int64), ("moves", ctypes.c_int64), ("vetoed", ctypes.c_int64),
+                ("interior", ctypes.c_int64), ("max_gain", ctypes.c_double), ("constant", ctypes.c_double),
+                ("probe_s", ctypes.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_destroy", "mvgpu_get_unique_id",
            "mvgpu_comm_init", "mvgpu_upload_shard", "mvgpu_attach_shard_device", "mvgpu_generate_rgg_shard", "mvgpu_generate_rgg_shard_ex",
            "mvgpu_download_shard", "mvgpu_louvain",
@@ -61,7 +70,8 @@ EXPORTS = ["mvgpu_last_error", "mvgpu_device_count", "mvgpu_create", "mvgpu_dest
            "mvgpu_get_timings", "mvgpu_get_scan_times", "mvgpu_get_constant", "mvgpu_get_shard_info", "mvgpu_dist_louvain_method",
            "mvgpu_set_initial_communities", "mvgpu_get_converged", "mvgpu_evaluate_communities",
            "mvgpu_get_community_stats", "mvgpu_get_compact_communities", "mvgpu_update_shard", "mvgpu_split_communities",
-           "mvgpu_compare_communities", "mvgpu_get_community_matches", "mvgpu_set_movable", "mvgpu_get_movable"]
+           "mvgpu_compare_communities", "mvgpu_get_community_matches", "mvgpu_set_movable", "mvgpu_get_movable",
+           "mvgpu_probe_communities"]
 
 _lib = None
 
@@ -99,6 +109,8 @@ def lib():
         L.mv_split_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(SplitReport)]
         L.mvgpu_compare_communities.argtypes = [vp, vp, vp, ctypes.POINTER(CompareReport)]
         L.mv_compare_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(CompareReport)]
+        L.mvgpu_probe_communities.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(ProbeReport)]
+        L.mv_probe_refused.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(ProbeReport)]
         L.mvgpu_get_community_matches.argtypes = [vp, vp, vp, vp, vp]
         L.mvgpu_get_compact_communities.argtypes = [vp, vp]
         L.mvgpu_upload_shard32.argtypes = [vp, ctypes.c_int32, vp, ctypes.c_int32, ctypes.c_int32, vp, vp]
@@ -366,6 +378,29 @@ class LouvainGPU:
         _ck(lib().mvgpu_compare_communities(self._h, None if bufs[0] is None else bufs[0].ctypes.data, bufs[1].ctypes.data,
                                             ctypes.byref(rep)))
         return rep.as_dict()
+
+    def probe(self, comm=None):
+        """What every vertex would do under the Louvain rule from an assignment (DESIGN.md §3.15), without moving anything.
+        `comm` takes the form evaluate() takes; None probes what the last louvain() returned.  Collective, with
+        evaluate()'s error rules.  Returns (report, target, best, gain): mvgpu_probe_report as a dict (global counts), and
+        this rank's lnv entries of the decision (int64), the best candidate community (int64, -1 without one) and its
+        gain (float64, -inf without one)."""
+        rep = ProbeReport()
+        n = max(self.lnv, 1)
+        target, best, gain = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(n, np.float64)
+        outs = (target.ctypes.data, best.ctypes.data, gain.ctypes.data)
+        if comm is None:
+            _ck(lib().mvgpu_probe_communities(self._h, None, *outs, ctypes.byref(rep)))
+        else:
+            comm = np.ascontiguousarray(comm, dtype=np.int64)
+            if comm.ndim != 1 or comm.size != self.lnv:
+                # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
+                why = f"assignment has {comm.size} entries, the shard has lnv = {self.lnv}"
+                _ck(lib().mv_probe_refused(self._h, why.encode(), ctypes.byref(rep)))
+                raise AssertionError("unreachable: a refused probe fails")
+            buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
+            _ck(lib().mvgpu_probe_communities(self._h, buf.ctypes.data, *outs, ctypes.byref(rep)))
+        return rep.as_dict(), target[:self.lnv], best[:self.lnv], gain[:self.lnv]
 
     def community_matches(self):
         """Per community of x in the last compare_communities(): entry s describes community parts[rank] + s.  Returns a
