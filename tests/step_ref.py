@@ -91,9 +91,25 @@ class Graph:
         return np.zeros(self.nv, bool) if heavy_deg is None else self.deg > heavy_deg
 
 
-def gain(eiy, eix, k, ay, ax, c):
-    """dspl.hpp:212 with the reference's association, elementwise in fp64 (numpy does not contract to FMA)."""
-    return 2.0 * (eiy - eix) - ((2.0 * k) * (ay - ax)) * c
+def fl32(x):
+    """Round to float and back (round to nearest even), elementwise."""
+    return np.asarray(x, np.float64).astype(np.float32).astype(np.float64)
+
+
+def gain(eiy, eix, k, ay, ax, c, f32=False):
+    """dspl.hpp:212 with the reference's association, elementwise in fp64 (numpy does not contract to FMA).
+    f32: the reference's USE_32_BIT_GRAPH build, where GraphWeight is float: (eiy - eix) and (ay - ax) are float
+    subtractions, the 2.0 literals carry the rest in double, and `GraphWeight curGain` rounds the result to float
+    (gain_of in kernels.cuh).  The inputs must be float values (below 2^24 units every sum is)."""
+    if not f32:
+        return 2.0 * (eiy - eix) - ((2.0 * k) * (ay - ax)) * c
+    return fl32(2.0 * fl32(eiy - eix) - ((2.0 * k) * fl32(ay - ax)) * c)
+
+
+def constant32(c):
+    """The float build's 1/(2m) from the double one: (float)(1.0 / (float)2m) (dspl.hpp:129).  For 2m below 2^24
+    (float)2m is 2m itself, so this is c rounded to float."""
+    return float(fl32(c))
 
 
 def _pairs(G, X, edge_order=None):
@@ -112,10 +128,16 @@ def _comm(G, X, vertex_order=None):
     return size, a
 
 
-def step(G, X, c, edge_order=None, vertex_order=None):
+def step(G, X, c, edge_order=None, vertex_order=None, f32=False, f32_constant=True):
     """fp64 mode.  edge_order / vertex_order (permutations, default the identity) reorder the counter sums and the
     community degree sums, for checking the certificate against other orders.  Returns dict(target, moved, size, a,
-    pairs = (v, y, gain) of every candidate, sorted by (v, y))."""
+    pairs = (v, y, gain) of every candidate, sorted by (v, y)).
+    f32: the USE_32_BIT_GRAPH build's step -- gain()'s three float roundings and the float constant constant32(c) --
+    exact where every sum stays below 2^24 units (the sums here are then the float build's values).  The equal-gain
+    rule is unchanged and now sees the float gains.  f32_constant=False keeps the double c with the float gains (to find
+    graphs where the constant's rounding alone decides)."""
+    if f32 and f32_constant:
+        c = constant32(c)
     X = np.asarray(X, np.int64)
     pv, pc, e, _cnt = _pairs(G, X, edge_order)
     own = pc == X[pv]
@@ -125,7 +147,7 @@ def step(G, X, c, edge_order=None, vertex_order=None):
     eix = w0 - G.sl
     ax = a[X] - G.k
     cv, cy, ce = pv[~own], pc[~own], e[~own]
-    g = gain(ce, eix[cv], G.k[cv], a[cy], ax[cv], c)
+    g = gain(ce, eix[cv], G.k[cv], a[cy], ax[cv], c, f32)
     pairs = (cv, cy, g)
     T = X.copy()
     pos = g > 0.0

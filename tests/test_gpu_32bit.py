@@ -34,9 +34,11 @@ def shards32(case):
     return parts.astype(np.int32), out
 
 
-def run32(case, **opts):
+def run32(case, thresh=1.0e-6, sharded=None, **opts):
+    """One float-build run of case on len(shards) ranks sharing device 0 (threads, host transport); sharded:
+    (parts, shards) when the case is not one case_graph rebuilds."""
     from minivite_b200 import gpu as G
-    parts, sh = shards32(case)
+    parts, sh = sharded or shards32(case)
     world = len(sh)
     ident = G.get_unique_id()
     out, errs = [None] * world, []
@@ -52,7 +54,7 @@ def run32(case, **opts):
             if world > 1:
                 g.comm_init(ident)
             g.upload32(int(parts[-1]), parts, sh[rank][0], sh[rank][1])
-            mod, iters = g.louvain32()
+            mod, iters = g.louvain32(thresh=thresh)
             out[rank] = {"mod": mod, "iters": iters, "trace": g.trace(), "comm": g.communities32().astype(np.int64),
                          "unit": g.timings()["unit_weight"]}
             g.close()
