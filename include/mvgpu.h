@@ -17,6 +17,18 @@
  * wrapper turns a failure into the reference's MPI_Abort(-99) behaviour).  A context must be driven
  * by one host thread at a time.  The library never falls back to a CPU implementation: without a
  * usable CUDA device every compute entry point fails.
+ *
+ * Per-vertex and per-community arrays in host or device memory (DESIGN.md §3.16).  Every array pointer of
+ * mvgpu_set_initial_communities, mvgpu_evaluate_communities, mvgpu_split_communities, mvgpu_probe_communities,
+ * mvgpu_compare_communities, mvgpu_set_movable, mvgpu_get_movable, mvgpu_update_shard, mvgpu_get_communities,
+ * mvgpu_get_compact_communities, mvgpu_get_community_stats and mvgpu_get_community_matches may be pageable or pinned host
+ * memory, or device (or managed) memory of the context's device; each pointer is classified on its own with
+ * cudaPointerGetAttributes, so ranks, and the two arrays of a compare, may differ in kind.  Device memory of another
+ * device is refused with a message naming both devices; in a collective call that refusal fails every rank, like a bad
+ * id.  Inputs are read on the library's stream after the call begins (the caller must have finished writing them) and
+ * are copied or consumed before it returns, never retained.  Outputs are complete when the call returns.  Every other
+ * message, and the meaning of NULL, is the same in both forms.  The 32-bit surface, mvgpu_upload_shard and
+ * mvgpu_download_shard take host arrays only.
  */
 #ifndef MVGPU_H
 #define MVGPU_H
@@ -111,7 +123,7 @@ int mvgpu_generate_rgg_shard_ex(mvgpu_ctx *ctx, int64_t nv_global, int unit_weig
 /* Copy the shard's reference-format arrays (lnv+1 offsets, lne 16-byte records) back to the host. */
 int mvgpu_download_shard(mvgpu_ctx *ctx, int64_t *edge_indices, void *edge_list);
 /* Change the shard in place on the device (DESIGN.md §3.11): n_del deletions (del_src[i], del_dst[i]) and n_ins
- * insertions (ins_src[i], ins_dst[i], ins_weight[i]), host arrays in global ids, src owned by this rank.  Per row:
+ * insertions (ins_src[i], ins_dst[i], ins_weight[i]), arrays in global ids, src owned by this rank.  Per row:
  * every old record whose tail is the dst of a deletion of that row is dropped (parallel records included; deletions
  * match old records only, so delete + insert of one pair replaces its weight); the insertions, stably sorted by dst,
  * are merged into the surviving records by "next old record while its tail <= the next insertion's dst, else the

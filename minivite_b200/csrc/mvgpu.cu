@@ -161,8 +161,9 @@ struct mvgpu_ctx {
   DevBuf<int32_t> in_tails32;
   DevBuf<Edge16> raw_ring;             // compact upload: raw chunks narrowed on the device (two slots)
   long long raw_chunks = 0;
-  DevBuf<long long> wide;
-  void *h_bounce[2] = {nullptr, nullptr};
+  DevBuf<long long> wide;              // int64 per-vertex arrays on their way to or from host memory
+  void *h_bounce[2] = {nullptr, nullptr};   // pinned chunks between wide and pageable host arrays, both ways
+  DevBuf<unsigned long long> take_bad; // k_take_ids: the smallest local index of a bad id
   const int32_t *d_tails32 = nullptr;
   long long in_nremote = 0;
   void *h_stage = nullptr;
@@ -1340,6 +1341,138 @@ __global__ void k_widen(const int32_t *in, long long n, long long *out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = in[i];
 }
 
+// ---- caller arrays in host or device memory (DESIGN.md §3.16) -------------------------------------------------------
+// The one range check of caller community ids, for both forms: ids[i] in [0, nv) narrowed to out[i]; *bad = the smallest
+// i whose id lies outside (left at its preset ~0 when every id is good).
+__global__ void __launch_bounds__(256) k_take_ids(const long long *ids, long long n, long long nv, int32_t *out,
+                                                  unsigned long long *bad) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long v = ids[i];
+    if (v < 0 || v >= nv) atomicMin(bad, (unsigned long long)i);
+    out[i] = (int32_t)v;
+  }
+}
+
+// a movable set as 0 / 1 (may run in place)
+__global__ void __launch_bounds__(256) k_mask01(const uint8_t *in, long long n, uint8_t *out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = in[i] != 0;
+}
+
+// Where a caller's array lives.  Each pointer is classified on its own: pageable or pinned host memory takes the host
+// form, device or managed memory of the context's device the device form.
+enum class Where { Pageable, Pinned, Device };
+
+// p's class in w; device memory of another device is refused: the message ("" if none) names the array as `name`
+std::string locate(const mvgpu_ctx *c, const void *p, const char *name, Where &w) {
+  w = Where::Pageable;
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {   // not known to CUDA: plain host memory
+    cudaGetLastError();
+    return "";
+  }
+  if (a.type == cudaMemoryTypeHost) w = Where::Pinned;
+  if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) {
+    if (a.device != c->device)
+      return std::string(name) + " is memory of device " + std::to_string(a.device) + ", the context's device is " +
+             std::to_string(c->device);
+    w = Where::Device;
+  }
+  return "";
+}
+
+constexpr long long kBounce = 4LL << 20;       // int64 entries per pinned bounce buffer (32 MB)
+
+int bounce_buffers(mvgpu_ctx *c) {
+  for (int b = 0; b < 2; b++)
+    if (!c->h_bounce[b]) CK(cudaMallocHost(&c->h_bounce[b], kBounce * sizeof(long long)));
+  return 0;
+}
+
+// n int64 of pageable host memory -> c->wide, in chunks through the two pinned bounce buffers (full PCIe rate instead of
+// the driver's staged pageable path): the reverse of mvgpu_get_communities.  Asynchronous; the source may change once
+// this returns.
+int stage_pageable(mvgpu_ctx *c, const int64_t *src, long long n) {
+  TRY(bounce_buffers(c));
+  cudaEvent_t ev[2] = {get_event(c, 0), get_event(c, 1)};
+  long long off = 0;
+  for (int k = 0; off < n; k++) {
+    const int b = k & 1;
+    const long long m = std::min(kBounce, n - off);
+    CK(cudaEventSynchronize(ev[b]));           // the copy out of this buffer two chunks ago (or in an earlier call) is done
+    memcpy(c->h_bounce[b], src + off, sizeof(long long) * m);
+    CK(cudaMemcpyAsync(c->wide.p + off, c->h_bounce[b], sizeof(long long) * m, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaEventRecord(ev[b], c->stream));
+    off += m;
+  }
+  return 0;
+}
+
+// The caller's lnv community ids (host or device memory, named `name` in a refusal) as int32 in dst, on the device.  A
+// finding goes into err ("" if none), prefixed by `who`: a refused pointer, or the smallest local index with an id
+// outside [0, nv) and that id.  The return value reports CUDA failures only.  Synchronous: the ids are read before it
+// returns.
+int take_ids(mvgpu_ctx *c, const int64_t *ids, const char *who, const char *name, int32_t *dst, std::string &err) {
+  Where w;
+  err = locate(c, ids, name, w);
+  if (!err.empty()) {
+    err = std::string(who) + ": " + err;
+    return 0;
+  }
+  const long long n = c->lnv;
+  if (n == 0) return 0;
+  cudaStream_t s = c->stream;
+  const long long *src = reinterpret_cast<const long long *>(ids);
+  if (w != Where::Device) {
+    TRY(c->wide.ensure(n));
+    if (w == Where::Pinned) CK(cudaMemcpyAsync(c->wide.p, ids, sizeof(long long) * n, cudaMemcpyHostToDevice, s));
+    else TRY(stage_pageable(c, ids, n));
+    src = c->wide.p;
+  }
+  TRY(c->take_bad.ensure(1));
+  CK(cudaMemsetAsync(c->take_bad.p, 0xff, sizeof(unsigned long long), s));
+  k_take_ids<<<grid_for(n, 256, c->num_sms), 256, 0, s>>>(src, n, c->nv_global, dst, c->take_bad.p);
+  CK(cudaGetLastError());
+  unsigned long long bad = 0;
+  CK(cudaMemcpyAsync(&bad, c->take_bad.p, sizeof bad, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (bad < (unsigned long long)n) {
+    long long v = 0;
+    CK(cudaMemcpyAsync(&v, src + bad, sizeof v, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    err = std::string(who) + ": community id " + std::to_string(v) + " of local vertex " + std::to_string(bad) +
+          " outside [0, nv)";
+  }
+  return 0;
+}
+
+// lnv int32 ids on the device -> the caller's int64 array (class w): widened straight into device memory, through wide
+// and one copy into host memory.  Synchronous.
+int put_ids(mvgpu_ctx *c, const int32_t *src, int64_t *out, Where w) {
+  const long long n = c->lnv;
+  if (n == 0) return 0;
+  long long *dst = reinterpret_cast<long long *>(out);
+  if (w != Where::Device) {
+    TRY(c->wide.ensure(n));
+    dst = c->wide.p;
+  }
+  k_widen<<<grid_for(n, 256, c->num_sms), 256, 0, c->stream>>>(src, n, dst);
+  CK(cudaGetLastError());
+  if (w != Where::Device) CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+// The output arrays of a call (NULL ones skipped): the first refusal, "" if none; their classes in w
+std::string locate_all(const mvgpu_ctx *c, int n, const void *const *p, const char *const *name, Where *w) {
+  for (int k = 0; k < n; k++) {
+    w[k] = Where::Pageable;
+    if (!p[k]) continue;
+    const std::string e = locate(c, p[k], name[k], w[k]);
+    if (!e.empty()) return e;
+  }
+  return "";
+}
+
 // What the getters and mv_layout_readback report about the last run.  setup_run overwrites these, so an evaluation
 // keeps a copy and puts it back.
 struct RunReport {
@@ -1420,19 +1553,7 @@ int evaluate_pass(mvgpu_ctx *c, const int32_t *X, mvgpu_quality *out) {
   return 0;
 }
 
-// the caller's community ids (lnv of them) as int32 in h; what is wrong with them ("" if nothing), prefixed by `who`
-std::string narrow_ids(const mvgpu_ctx *c, const int64_t *comm, const char *who, std::vector<int32_t> &h) {
-  h.resize((size_t)c->lnv);
-  for (long long i = 0; i < c->lnv; i++) {
-    if (comm[i] < 0 || comm[i] >= c->nv_global)
-      return std::string(who) + ": community id " + std::to_string((long long)comm[i]) + " of local vertex " + std::to_string(i) +
-             " outside [0, nv)";
-    h[i] = (int32_t)comm[i];
-  }
-  return "";
-}
-
-// The assignment an evaluation or a split reads: comm (validated and copied to eval_comm) or, for NULL, the last run's
+// The assignment an evaluation or a split reads: comm (validated and narrowed into eval_comm) or, for NULL, the last run's
 // result in caller order (resolved by the caller of this).  Local findings are not returned here: they go into ev.err,
 // prefixed by `who`, and join setup_run's input agreement, so that every rank fails together.  caller_err: a finding of
 // the caller's own (a binding that could not build the array), which fails the call on every rank like a bad id.
@@ -1443,14 +1564,9 @@ int take_assignment(mvgpu_ctx *c, const int64_t *comm, const char *who, const ch
   else if (c->f32) ev.err = w + ": not for a shard uploaded with mvgpu_upload_shard32";
   else if (!comm && !c->run_on_shard) ev.err = w + ": NULL " + verb + " the last mvgpu_louvain result, and there is none on this shard";
   else if (comm) {
-    std::vector<int32_t> h;
-    ev.err = narrow_ids(c, comm, who, h);
-    if (ev.err.empty()) {
-      TRY(c->eval_comm.ensure(c->lnv));
-      if (c->lnv) CK(cudaMemcpyAsync(c->eval_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice, c->stream));
-      CK(cudaStreamSynchronize(c->stream));
-      ev.X = c->eval_comm.p;
-    }
+    TRY(c->eval_comm.ensure(c->lnv));
+    TRY(take_ids(c, comm, who, "comm", c->eval_comm.p, ev.err));
+    if (ev.err.empty()) ev.X = c->eval_comm.p;
   } else {
     ev.X = c->final_orig.p;
   }
@@ -1560,17 +1676,13 @@ int split(mvgpu_ctx *c, const int64_t *comm, int64_t *out, mvgpu_split_report *r
   if (c->run_on_shard) TRY(final_in_caller_order(c));   // as in evaluate: setup_run overwrites comm_a
   EvalSetup ev;
   ev.split = true;
-  TRY(take_assignment(c, comm, "mvgpu_split_communities", "splits", caller_err, ev));
+  Where w;
+  const std::string out_err = locate(c, out, "out", w);   // a refused output fails every rank, like a bad id
+  TRY(take_assignment(c, comm, "mvgpu_split_communities", "splits", caller_err ? caller_err : out_err.empty() ? nullptr : out_err.c_str(), ev));
   mvgpu_split_report r;
   memset(&r, 0, sizeof r);
   TRY(assignment_pass(c, ev, [&] { return split_pass(c, &r); }, r.split_s));
-  if (c->lnv > 0) {
-    TRY(c->wide.ensure(c->lnv));
-    k_widen<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(c->split_lab.p, c->lnv, c->wide.p);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * c->lnv, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-  }
+  TRY(put_ids(c, c->split_lab.p, out, w));
   *rep = r;
   return 0;
 }
@@ -1631,23 +1743,18 @@ int probe(mvgpu_ctx *c, const int64_t *comm, int64_t *target, int64_t *best, dou
   if (c->run_on_shard) TRY(final_in_caller_order(c));   // as in evaluate: setup_run overwrites comm_a
   EvalSetup ev;
   ev.probe = true;
-  TRY(take_assignment(c, comm, "mvgpu_probe_communities", "probes", caller_err, ev));
+  const void *outs[3] = {target, best, gain};
+  const char *names[3] = {"target", "best", "gain"};
+  Where w[3];
+  const std::string out_err = locate_all(c, 3, outs, names, w);   // a refused output fails every rank, like a bad id
+  TRY(take_assignment(c, comm, "mvgpu_probe_communities", "probes", caller_err ? caller_err : out_err.empty() ? nullptr : out_err.c_str(), ev));
   mvgpu_probe_report r;
   memset(&r, 0, sizeof r);
   TRY(assignment_pass(c, ev, [&] { return probe_pass(c, r); }, r.probe_s));
-  const long long lnv = c->lnv;
-  if (lnv > 0) {
-    int32_t *src[2] = {c->probe_tgt.p, c->probe_best.p};
-    int64_t *dst[2] = {target, best};
-    for (int k = 0; k < 2; k++) {
-      if (!dst[k]) continue;
-      TRY(c->wide.ensure(lnv));
-      k_widen<<<grid_for(lnv, 256, c->num_sms), 256, 0, c->stream>>>(src[k], lnv, c->wide.p);
-      CK(cudaGetLastError());
-      CK(cudaMemcpyAsync(dst[k], c->wide.p, sizeof(long long) * lnv, cudaMemcpyDeviceToHost, c->stream));
-      CK(cudaStreamSynchronize(c->stream));
-    }
-    if (gain) CK(cudaMemcpyAsync(gain, c->probe_gain.p, sizeof(double) * lnv, cudaMemcpyDeviceToHost, c->stream));
+  if (target) TRY(put_ids(c, c->probe_tgt.p, target, w[0]));
+  if (best) TRY(put_ids(c, c->probe_best.p, best, w[1]));
+  if (gain && c->lnv > 0) {
+    CK(cudaMemcpyAsync(gain, c->probe_gain.p, sizeof(double) * c->lnv, cudaMemcpyDefault, c->stream));
     CK(cudaStreamSynchronize(c->stream));
   }
   *rep = r;
@@ -1867,14 +1974,15 @@ int compare(mvgpu_ctx *c, const int64_t *x, const int64_t *y, mvgpu_compare_repo
   CK(cudaSetDevice(c->device));
   const std::string who = "mvgpu_compare_communities";
   std::string err;
-  std::vector<int32_t> hx, hy;
+  const long long lnv = c->lnv;
   if (caller_err) err = who + ": " + caller_err;
   else if (c->f32) err = who + ": not for a shard uploaded with mvgpu_upload_shard32";
   else if (!y) err = who + ": y must not be NULL";
   else if (!x && !c->run_on_shard) err = who + ": NULL x compares the last mvgpu_louvain result, and there is none on this shard";
   else {
-    if (x) err = narrow_ids(c, x, who.c_str(), hx);
-    if (err.empty()) err = narrow_ids(c, y, who.c_str(), hy);
+    TRY(c->cmp_x.ensure(lnv)); TRY(c->cmp_y.ensure(lnv));
+    if (x) TRY(take_ids(c, x, who.c_str(), "x", c->cmp_x.p, err));
+    if (err.empty()) TRY(take_ids(c, y, who.c_str(), "y", c->cmp_y.p, err));
   }
   // the call's first collective: one rank's finding fails every rank before any data moves
   if (c->nranks > 1) {
@@ -1889,11 +1997,7 @@ int compare(mvgpu_ctx *c, const int64_t *x, const int64_t *y, mvgpu_compare_repo
   }
   if (!err.empty()) return fail(err);
   cudaStream_t s = c->stream;
-  const long long lnv = c->lnv;
   if (!x) TRY(final_in_caller_order(c));       // one-rank runs leave it unresolved
-  TRY(c->cmp_x.ensure(lnv)); TRY(c->cmp_y.ensure(lnv));
-  if (x && lnv) CK(cudaMemcpyAsync(c->cmp_x.p, hx.data(), sizeof(int32_t) * lnv, cudaMemcpyHostToDevice, s));
-  if (lnv) CK(cudaMemcpyAsync(c->cmp_y.p, hy.data(), sizeof(int32_t) * lnv, cudaMemcpyHostToDevice, s));
   mvgpu_compare_report r;
   memset(&r, 0, sizeof r);
   cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
@@ -1949,33 +2053,43 @@ int merge_records(mvgpu_ctx *c, long long n, const long long *rowptr, const Edge
   return 0;
 }
 
-// This rank's part of mvgpu_update_shard before the agreement: the batch to the device, validated, sorted and merged
-// into nrow / nedges.  Leaves the shard itself as it is.
+// A batch array of n entries as the kernels read it: the caller's own when it is device memory (dev), else a copy in buf
+template <typename T>
+int batch_array(mvgpu_ctx *c, const T *p, long long n, bool dev, DevBuf<T> &buf, const T *&out) {
+  out = p;
+  if (dev) return 0;
+  TRY(buf.ensure(n));
+  if (n) CK(cudaMemcpyAsync(buf.p, p, sizeof(T) * n, cudaMemcpyHostToDevice, c->stream));
+  out = buf.p;
+  return 0;
+}
+
+// This rank's part of mvgpu_update_shard before the agreement: the batch to the device (dev[k]: array k, in the order of
+// the arguments, is device memory and is read in place), validated, sorted and merged into nrow / nedges.  Leaves the
+// shard itself as it is.
 int update_prepare(mvgpu_ctx *c, long long n_del, const int64_t *del_src, const int64_t *del_dst, long long n_ins,
-                   const int64_t *ins_src, const int64_t *ins_dst, const double *ins_weight, DevBuf<long long> &nrow,
-                   DevBuf<Edge16> &nedges, long long *lne_out) {
+                   const int64_t *ins_src, const int64_t *ins_dst, const double *ins_weight, const bool *dev,
+                   DevBuf<long long> &nrow, DevBuf<Edge16> &nedges, long long *lne_out) {
   cudaStream_t s = c->stream;
   const int nsm = c->num_sms;
   DevBuf<long long> dsrc, ddst, isrc, idst;
   DevBuf<double> iw;
   DevBuf<unsigned long long> dkey, dkey_s, ikey, ikey_s;
   DevBuf<unsigned int> iidx, iidx_s, bad;
-  TRY(dsrc.ensure(n_del)); TRY(ddst.ensure(n_del)); TRY(dkey.ensure(n_del)); TRY(dkey_s.ensure(n_del));
-  TRY(isrc.ensure(n_ins)); TRY(idst.ensure(n_ins)); TRY(iw.ensure(n_ins)); TRY(ikey.ensure(n_ins)); TRY(ikey_s.ensure(n_ins));
+  TRY(dkey.ensure(n_del)); TRY(dkey_s.ensure(n_del));
+  TRY(ikey.ensure(n_ins)); TRY(ikey_s.ensure(n_ins));
   TRY(iidx.ensure(n_ins)); TRY(iidx_s.ensure(n_ins)); TRY(bad.ensure(1));
-  if (n_del) {
-    CK(cudaMemcpyAsync(dsrc.p, del_src, sizeof(long long) * n_del, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ddst.p, del_dst, sizeof(long long) * n_del, cudaMemcpyHostToDevice, s));
-  }
-  if (n_ins) {
-    CK(cudaMemcpyAsync(isrc.p, ins_src, sizeof(long long) * n_ins, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(idst.p, ins_dst, sizeof(long long) * n_ins, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(iw.p, ins_weight, sizeof(double) * n_ins, cudaMemcpyHostToDevice, s));
-  }
+  const long long *ds, *dd, *is, *id;
+  const double *w;
+  TRY(batch_array(c, reinterpret_cast<const long long *>(del_src), n_del, dev[0], dsrc, ds));
+  TRY(batch_array(c, reinterpret_cast<const long long *>(del_dst), n_del, dev[1], ddst, dd));
+  TRY(batch_array(c, reinterpret_cast<const long long *>(ins_src), n_ins, dev[2], isrc, is));
+  TRY(batch_array(c, reinterpret_cast<const long long *>(ins_dst), n_ins, dev[3], idst, id));
+  TRY(batch_array(c, ins_weight, n_ins, dev[4], iw, w));
   CK(cudaMemsetAsync(bad.p, 0, sizeof(unsigned int), s));
   k_rowptr_check<<<grid_for(c->lnv + 1, 256, nsm), 256, 0, s>>>(c->d_rowptr64, c->lnv, c->lne, bad.p);
-  if (n_del) k_batch_keys<<<grid_for(n_del, 256, nsm), 256, 0, s>>>(dsrc.p, ddst.p, n_del, c->base, c->bound, c->nv_global, dkey.p, nullptr, bad.p);
-  if (n_ins) k_batch_keys<<<grid_for(n_ins, 256, nsm), 256, 0, s>>>(isrc.p, idst.p, n_ins, c->base, c->bound, c->nv_global, ikey.p, iidx.p, bad.p);
+  if (n_del) k_batch_keys<<<grid_for(n_del, 256, nsm), 256, 0, s>>>(ds, dd, n_del, c->base, c->bound, c->nv_global, dkey.p, nullptr, bad.p);
+  if (n_ins) k_batch_keys<<<grid_for(n_ins, 256, nsm), 256, 0, s>>>(is, id, n_ins, c->base, c->bound, c->nv_global, ikey.p, iidx.p, bad.p);
   CK(cudaGetLastError());
   unsigned int hbad = 0;
   CK(cudaMemcpyAsync(&hbad, bad.p, sizeof hbad, cudaMemcpyDeviceToHost, s));
@@ -1987,7 +2101,7 @@ int update_prepare(mvgpu_ctx *c, long long n_del, const int64_t *del_src, const 
   // batch order
   if (n_del) TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortKeys(t, tb, dkey.p, dkey_s.p, (int)n_del, 0, 62, s); }));
   if (n_ins) TRY(cub_run(c, [&](void *t, size_t &tb) { return cub::DeviceRadixSort::SortPairs(t, tb, ikey.p, ikey_s.p, iidx.p, iidx_s.p, (int)n_ins, 0, 62, s); }));
-  return merge_records(c, c->lnv, c->d_rowptr64, c->d_edges, c->lne, dkey_s.p, n_del, ikey_s.p, iidx_s.p, iw.p, n_ins, nrow, nedges, lne_out);
+  return merge_records(c, c->lnv, c->d_rowptr64, c->d_edges, c->lne, dkey_s.p, n_del, ikey_s.p, iidx_s.p, w, n_ins, nrow, nedges, lne_out);
 }
 
 }  // namespace
@@ -2437,11 +2551,20 @@ int mvgpu_update_shard(mvgpu_ctx *c, int64_t n_del, const int64_t *del_src, cons
   else if (n_del < 0 || n_ins < 0) err = "negative batch size";
   else if (n_del >= (1LL << 31) || n_ins >= (1LL << 31)) err = "batch too large: fewer than 2^31 deletions and 2^31 insertions per call";
   else if ((n_del && (!del_src || !del_dst)) || (n_ins && (!ins_src || !ins_dst || !ins_weight))) err = "null batch array";
+  bool dev[5] = {};
+  if (err.empty()) {                            // the arrays of an empty side are not read
+    const void *arr[5] = {n_del ? del_src : nullptr, n_del ? del_dst : nullptr, n_ins ? ins_src : nullptr,
+                          n_ins ? ins_dst : nullptr, n_ins ? ins_weight : nullptr};
+    const char *names[5] = {"del_src", "del_dst", "ins_src", "ins_dst", "ins_weight"};
+    Where w[5];
+    err = locate_all(c, 5, arr, names, w);
+    for (int k = 0; k < 5; k++) dev[k] = w[k] == Where::Device;
+  }
   if (!err.empty()) err = "mvgpu_update_shard: " + err;
   DevBuf<long long> nrow;
   DevBuf<Edge16> nedges;
   long long lne2 = 0;
-  if (err.empty() && update_prepare(c, n_del, del_src, del_dst, n_ins, ins_src, ins_dst, ins_weight, nrow, nedges, &lne2)) err = g_err;
+  if (err.empty() && update_prepare(c, n_del, del_src, del_dst, n_ins, ins_src, ins_dst, ins_weight, dev, nrow, nedges, &lne2)) err = g_err;
   if (c->nranks > 1) {
     TRY(c->scratch.ensure(sizeof(Scalars)));
     long long any = err.empty() ? 0 : 1;
@@ -2476,12 +2599,13 @@ int mvgpu_set_initial_communities(mvgpu_ctx *c, const int64_t *comm) {
   if (!c) return fail("null argument");
   if (!comm) { c->have_init = false; return 0; }
   if (!c->have_graph) return fail("mvgpu_set_initial_communities: no shard yet (upload, attach or generate one first)");
-  std::vector<int32_t> h;
-  const std::string err = narrow_ids(c, comm, "mvgpu_set_initial_communities", h);
-  if (!err.empty()) return fail(err);
   CK(cudaSetDevice(c->device));
-  TRY(c->init_comm.ensure(c->lnv));
-  if (c->lnv) CK(cudaMemcpy(c->init_comm.p, h.data(), sizeof(int32_t) * c->lnv, cudaMemcpyHostToDevice));
+  // staged in eval_comm, which only lives inside one call, so that a refused array leaves the current one in place
+  TRY(c->eval_comm.ensure(c->lnv));
+  std::string err;
+  TRY(take_ids(c, comm, "mvgpu_set_initial_communities", "comm", c->eval_comm.p, err));
+  if (!err.empty()) return fail(err);
+  c->init_comm.swap(c->eval_comm);
   c->have_init = true;
   return 0;
 }
@@ -2489,13 +2613,25 @@ int mvgpu_set_initial_communities(mvgpu_ctx *c, const int64_t *comm) {
 int mvgpu_set_movable(mvgpu_ctx *c, const uint8_t *mask) {
   if (!c) return fail("null argument");
   if (mask && !c->have_graph) return fail("mvgpu_set_movable: no shard yet (upload, attach or generate one first)");
+  Where w = Where::Pageable;
+  if (mask) {
+    CK(cudaSetDevice(c->device));
+    const std::string err = locate(c, mask, "mask", w);
+    if (!err.empty()) return fail("mvgpu_set_movable: " + err);
+  }
   c->mov_out_valid = false;
   c->peers_ready = false;          // a masked run with the frontier option exports two more arrays
   if (!mask) { c->have_mov = false; return 0; }
-  CK(cudaSetDevice(c->device));
   TRY(c->mov_in.ensure(c->lnv));
   if (c->lnv) {                                // on the context's stream, behind any run still reading mov_in
-    CK(cudaMemcpyAsync(c->mov_in.p, mask, c->lnv, cudaMemcpyHostToDevice, c->stream));
+    const uint8_t *src = mask;
+    if (w != Where::Device) {
+      CK(cudaMemcpyAsync(c->mov_in.p, mask, c->lnv, cudaMemcpyHostToDevice, c->stream));
+      src = c->mov_in.p;
+    }
+    // kept as 0 / 1, the form mvgpu_get_movable returns (the run's kernels read any nonzero byte as movable)
+    k_mask01<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(src, c->lnv, c->mov_in.p);
+    CK(cudaGetLastError());
     CK(cudaStreamSynchronize(c->stream));
   }
   c->have_mov = true;
@@ -2505,16 +2641,20 @@ int mvgpu_set_movable(mvgpu_ctx *c, const uint8_t *mask) {
 int mvgpu_get_movable(mvgpu_ctx *c, uint8_t *out) {
   if (!c || !out) return fail("null argument");
   if (!c->have_graph) return fail("mvgpu_get_movable: no shard yet (upload, attach or generate one first)");
-  if (c->lnv == 0) return 0;
   CK(cudaSetDevice(c->device));
+  Where w;
+  const std::string err = locate(c, out, "out", w);
+  if (!err.empty()) return fail("mvgpu_get_movable: " + err);
+  if (c->lnv == 0) return 0;
   // on the context's stream: the run leaves k_movable_out queued behind its end event (and c->stream does not
   // synchronise with the legacy default stream)
-  if (c->mov_out_valid || c->have_mov) {
-    CK(cudaMemcpyAsync(out, c->mov_out_valid ? c->mov_out.p : c->mov_in.p, c->lnv, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    if (!c->mov_out_valid)                     // the set as given, as 0 / 1
-      for (long long i = 0; i < c->lnv; i++) out[i] = out[i] != 0;
-  } else memset(out, 1, (size_t)c->lnv);
+  if (c->mov_out_valid || c->have_mov)
+    CK(cudaMemcpyAsync(out, c->mov_out_valid ? c->mov_out.p : c->mov_in.p, c->lnv, cudaMemcpyDefault, c->stream));
+  else if (w == Where::Device)
+    CK(cudaMemsetAsync(out, 1, (size_t)c->lnv, c->stream));
+  else
+    memset(out, 1, (size_t)c->lnv);
+  CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
 
@@ -2571,8 +2711,13 @@ int mvgpu_get_community_matches(mvgpu_ctx *c, int64_t *size, int64_t *best, int6
   CK(cudaSetDevice(c->device));
   const size_t n = (size_t)c->lnv;
   int64_t *dst[4] = {size, best, overlap, best_size};
+  const void *arr[4] = {size, best, overlap, best_size};
+  const char *names[4] = {"size", "best", "overlap", "best_size"};
+  Where w[4];
+  const std::string err = locate_all(c, 4, arr, names, w);
+  if (!err.empty()) return fail("mvgpu_get_community_matches: " + err);
   for (int k = 0; k < 4; k++)
-    if (dst[k] && n) CK(cudaMemcpyAsync(dst[k], c->cmp_match.p + k * n, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
+    if (dst[k] && n) CK(cudaMemcpyAsync(dst[k], c->cmp_match.p + k * n, sizeof(long long) * n, cudaMemcpyDefault, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -2582,9 +2727,14 @@ int mvgpu_get_community_stats(mvgpu_ctx *c, int64_t *size, double *volume, doubl
   if (!c->eval_on_shard) return fail("no evaluation of this shard yet (mvgpu_evaluate_communities)");
   CK(cudaSetDevice(c->device));
   const size_t n = (size_t)c->lnv;
-  if (size && n) CK(cudaMemcpyAsync(size, c->q_size.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
-  if (volume && n) CK(cudaMemcpyAsync(volume, c->q_vol.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
-  if (internal && n) CK(cudaMemcpyAsync(internal, c->q_internal.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+  const void *arr[3] = {size, volume, internal};
+  const char *names[3] = {"size", "volume", "internal"};
+  Where w[3];
+  const std::string err = locate_all(c, 3, arr, names, w);
+  if (!err.empty()) return fail("mvgpu_get_community_stats: " + err);
+  if (size && n) CK(cudaMemcpyAsync(size, c->q_size.p, sizeof(long long) * n, cudaMemcpyDefault, c->stream));
+  if (volume && n) CK(cudaMemcpyAsync(volume, c->q_vol.p, sizeof(double) * n, cudaMemcpyDefault, c->stream));
+  if (internal && n) CK(cudaMemcpyAsync(internal, c->q_internal.p, sizeof(double) * n, cudaMemcpyDefault, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -2592,14 +2742,11 @@ int mvgpu_get_community_stats(mvgpu_ctx *c, int64_t *size, double *volume, doubl
 int mvgpu_get_compact_communities(mvgpu_ctx *c, int64_t *out) {
   if (!c || !out) return fail("null argument");
   if (!c->eval_on_shard) return fail("no evaluation of this shard yet (mvgpu_evaluate_communities)");
-  if (c->lnv == 0) return 0;
   CK(cudaSetDevice(c->device));
-  TRY(c->wide.ensure(c->lnv));
-  k_widen<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(c->q_lab.p, c->lnv, c->wide.p);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * c->lnv, cudaMemcpyDeviceToHost, c->stream));
-  CK(cudaStreamSynchronize(c->stream));
-  return 0;
+  Where w;
+  const std::string err = locate(c, out, "out", w);
+  if (!err.empty()) return fail("mvgpu_get_compact_communities: " + err);
+  return put_ids(c, c->q_lab.p, out, w);
 }
 
 int mvgpu_get_converged(mvgpu_ctx *c, int *converged) {
@@ -2624,23 +2771,19 @@ int mvgpu_get_communities_device(mvgpu_ctx *c, const int32_t **d_out) {
 int mvgpu_get_communities(mvgpu_ctx *c, int64_t *out) {
   if (!c || !out) return fail("null argument");
   if (!c->final_on_shard) return fail(kNoRunOnShard);
+  CK(cudaSetDevice(c->device));
+  Where w;
+  const std::string err = locate(c, out, "out", w);
+  if (!err.empty()) return fail("mvgpu_get_communities: " + err);
   if (c->lnv == 0) return 0;
   TRY(final_in_caller_order(c));
+  // device and pinned destinations are written by put_ids; pageable ones are copied through the pinned bounce buffers
+  // in chunks (full PCIe rate instead of the driver's staged pageable path)
+  if (w != Where::Pageable) return put_ids(c, c->final_orig.p, out, w);
   TRY(c->wide.ensure(c->lnv));
   k_widen<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(c->final_orig.p, c->lnv, c->wide.p);
-  // pageable destinations are copied through a pinned bounce buffer in chunks (full PCIe rate instead of the
-  // driver's staged pageable path); a pinned destination is detected and written directly
-  cudaPointerAttributes attr;
-  const bool pinned = cudaPointerGetAttributes(&attr, out) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-  cudaGetLastError();
-  if (pinned) {
-    CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * c->lnv, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    return 0;
-  }
-  const long long CH = 4LL << 20;                                  // 4 Mi entries = 32 MB per bounce buffer
-  for (int b = 0; b < 2; b++)
-    if (!c->h_bounce[b]) CK(cudaMallocHost(&c->h_bounce[b], CH * sizeof(long long)));
+  const long long CH = kBounce;
+  TRY(bounce_buffers(c));
   struct { long long off, n; } pend[2] = {{0, 0}, {0, 0}};
   cudaEvent_t ev[2] = {get_event(c, 0), get_event(c, 1)};
   long long off = 0;

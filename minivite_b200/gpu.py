@@ -3,9 +3,14 @@
 `dist_louvain_method(me, nprocs, shard, lower, thresh)` has the argument meaning of the reference's
 `distLouvainMethod` (dspl.hpp:1280-1283): it returns (modularity, iters).  There is NO CPU fallback:
 if the CUDA library is missing or no GPU is usable every call raises.
+
+Per-vertex inputs (assignments, masks, update batches) may be NumPy arrays or torch tensors; a CUDA tensor is read
+where it lies (DESIGN.md §3.16).  Per-vertex outputs are NumPy arrays, or torch tensors on the context's device with
+device=True.  torch is imported only when a tensor is passed or device=True.
 """
 import ctypes
 import os
+import sys
 
 import numpy as np
 
@@ -138,6 +143,54 @@ def _ck(rc):
         raise MvgpuError(lib().mvgpu_last_error().decode(errors="replace"))
 
 
+_NP = {"i8": np.int64, "u1": np.uint8, "f8": np.float64}
+_TORCH = {"i8": "int64", "u1": "uint8", "f8": "float64"}
+
+
+def _cuda_tensor(a):
+    t = sys.modules.get("torch")         # a caller holding a tensor has imported torch
+    return t is not None and isinstance(a, t.Tensor) and a.is_cuda
+
+
+class _Input:
+    """An input array as the C ABI reads it.  kind: "i8" (int64 ids), "u1" (a mask: nonzero = 1) or "f8" (float64).
+    A CUDA tensor is converted on its own device and passed as a device pointer once its current stream has been
+    synchronised (the library reads it on its own stream); a tensor on another device than the context's is passed
+    as well, and the library refuses it.  Anything else becomes a C-contiguous NumPy array.  An empty array passes a
+    one-element dummy of the same kind: a zero-length array has no address, and NULL means "no array"."""
+
+    def __init__(self, a, kind, flat=False):
+        if _cuda_tensor(a):
+            import torch
+            t = a.reshape(-1) if flat else a
+            t = (t != 0).to(torch.uint8) if kind == "u1" and t.dtype != torch.uint8 else t.to(getattr(torch, _TORCH[kind]))
+            t = t.contiguous()
+            self.ndim, self.size = t.dim(), t.numel()
+            self.arr = t if self.size else torch.zeros(1, dtype=t.dtype, device=t.device)
+            torch.cuda.current_stream(t.device).synchronize()
+            self.ptr = self.arr.data_ptr()
+        else:
+            x = np.ascontiguousarray(a)
+            x = x.reshape(-1) if flat else x
+            x = (x != 0).astype(np.uint8) if kind == "u1" and x.dtype != np.uint8 else np.ascontiguousarray(x, _NP[kind])
+            self.ndim, self.size = x.ndim, x.size
+            self.arr = x if x.size else np.zeros(1, _NP[kind])
+            self.ptr = self.arr.ctypes.data
+
+
+def _outputs(device, ctx_device, n, kinds):
+    """Output arrays of n entries (at least one, so that a pointer is never NULL on an empty rank): NumPy, or torch
+    tensors on the context's device (device=True), whose allocation the library's stream is ordered after."""
+    if not device:
+        out = [np.zeros(max(n, 1), _NP[k]) for k in kinds]
+        return out, [o.ctypes.data for o in out]
+    import torch
+    dev = torch.device("cuda", ctx_device)
+    out = [torch.empty(max(n, 1), dtype=getattr(torch, _TORCH[k]), device=dev) for k in kinds]
+    torch.cuda.current_stream(dev).synchronize()
+    return out, [o.data_ptr() for o in out]
+
+
 def device_count():
     n = lib().mvgpu_device_count()
     if n < 0:
@@ -232,24 +285,23 @@ class LouvainGPU:
         """Change the shard in place on the device (DESIGN.md §3.11): delete=(src, dst) drops every record (src, dst) of
         the shard, insert=(src, dst, w) merges new records in; global ids, src owned by this rank, both directions of an
         undirected edge given by the caller.  Collective with several ranks (pass None, None when a rank has no
-        changes).  Returns the new lne."""
-        def cols(t, dtypes, what):
+        changes).  Returns the new lne.  Each array may be a NumPy array or a torch tensor (CUDA tensors are read on the
+        device)."""
+        def cols(t, kinds, what):
             if t is None:
-                return [np.zeros(0, d) for d in dtypes]
-            if len(t) != len(dtypes):
-                raise ValueError(f"{what} takes {len(dtypes)} arrays")
-            out = [np.ascontiguousarray(a, dtype=d).reshape(-1) for a, d in zip(t, dtypes)]
-            if any(a.size != out[0].size for a in out):
+                return 0, [None] * len(kinds), []
+            if len(t) != len(kinds):
+                raise ValueError(f"{what} takes {len(kinds)} arrays")
+            arrs = [_Input(a, k, flat=True) for a, k in zip(t, kinds)]
+            if any(a.size != arrs[0].size for a in arrs):
                 raise ValueError(f"{what}: arrays of different lengths")
-            return out
-        ds, dd = cols(delete, (np.int64, np.int64), "delete")
-        is_, id_, iw = cols(insert, (np.int64, np.int64, np.float64), "insert")
-
-        def ptr(a):
-            return a.ctypes.data if a.size else None
+            n = arrs[0].size
+            return n, [a.ptr if n else None for a in arrs], arrs
+        n_del, (ds, dd), keep_del = cols(delete, ("i8", "i8"), "delete")
+        n_ins, (is_, id_, iw), keep_ins = cols(insert, ("i8", "i8", "f8"), "insert")
         lne = ctypes.c_int64(0)
-        _ck(lib().mvgpu_update_shard(self._h, ds.size, ptr(ds), ptr(dd), is_.size, ptr(is_), ptr(id_), ptr(iw),
-                                     ctypes.byref(lne)))
+        _ck(lib().mvgpu_update_shard(self._h, n_del, ds, dd, n_ins, is_, id_, iw, ctypes.byref(lne)))
+        del keep_del, keep_ins
         self._keep = None            # an attached shard's arrays are no longer read
         return lne.value
 
@@ -264,39 +316,37 @@ class LouvainGPU:
 
     def set_initial_communities(self, comm):
         """Start every later louvain() on this shard from `comm` (lnv global community ids in [0, nv), caller's vertex
-        numbering, e.g. what communities() returned) instead of singletons; None clears it.  A new upload / attach /
-        generate clears it too.  Resuming a run stopped by the stop_after option from its communities() with lower = its
-        modularity continues that run exactly."""
+        numbering, e.g. what communities() returned; a NumPy array or a torch tensor) instead of singletons; None clears
+        it.  The array is copied at call time.  A new upload / attach / generate clears it too.  Resuming a run stopped by
+        the stop_after option from its communities() with lower = its modularity continues that run exactly."""
         if comm is None:
             _ck(lib().mvgpu_set_initial_communities(self._h, None))
             return
-        comm = np.ascontiguousarray(comm, dtype=np.int64)
-        if comm.ndim != 1 or comm.size != self.lnv:
-            raise ValueError(f"initial assignment has {comm.size} entries, the shard has lnv = {self.lnv}")
-        buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
-        _ck(lib().mvgpu_set_initial_communities(self._h, buf.ctypes.data))
+        a = _Input(comm, "i8")
+        if a.ndim != 1 or a.size != self.lnv:
+            raise ValueError(f"initial assignment has {a.size} entries, the shard has lnv = {self.lnv}")
+        _ck(lib().mvgpu_set_initial_communities(self._h, a.ptr))
 
     def set_movable(self, mask):
         """Hold vertices in place (DESIGN.md §3.14): every later louvain() on this shard lets only the vertices with a
-        nonzero byte in `mask` (lnv entries, caller's vertex numbering) move; with the option frontier = 1 the set grows
-        from the vertices that move.  None clears it (everything movable); a new upload / attach / generate clears it too,
-        update_shard keeps it.  With several ranks every rank or none must set one."""
+        nonzero entry in `mask` (lnv entries, caller's vertex numbering, a NumPy array or a torch tensor) move; with the
+        option frontier = 1 the set grows from the vertices that move.  The mask is copied at call time.  None clears it
+        (everything movable); a new upload / attach / generate clears it too, update_shard keeps it.  With several ranks
+        every rank or none must set one."""
         if mask is None:
             _ck(lib().mvgpu_set_movable(self._h, None))
             return
-        mask = np.ascontiguousarray(mask)
-        if mask.ndim != 1 or mask.size != self.lnv:
-            raise ValueError(f"movable set has {mask.size} entries, the shard has lnv = {self.lnv}")
-        buf = (mask != 0).astype(np.uint8) if mask.dtype != np.uint8 else mask
-        if not buf.size:
-            buf = np.zeros(1, np.uint8)                          # an empty shard still passes a non-NULL array
-        _ck(lib().mvgpu_set_movable(self._h, buf.ctypes.data))
+        a = _Input(mask, "u1")
+        if a.ndim != 1 or a.size != self.lnv:
+            raise ValueError(f"movable set has {a.size} entries, the shard has lnv = {self.lnv}")
+        _ck(lib().mvgpu_set_movable(self._h, a.ptr))
 
-    def movable(self):
+    def movable(self, device=False):
         """The set the next iteration would use (uint8 0 / 1, lnv entries): after a run with a set, the set after its last
-        accepted iteration -- resume a stop_after checkpoint with it; otherwise the set as given, all ones without one."""
-        out = np.zeros(max(self.lnv, 1), np.uint8)
-        _ck(lib().mvgpu_get_movable(self._h, out.ctypes.data))
+        accepted iteration -- resume a stop_after checkpoint with it; otherwise the set as given, all ones without one.
+        device=True: a torch tensor on the context's device."""
+        (out,), (p,) = _outputs(device, self.device, self.lnv, ("u1",))
+        _ck(lib().mvgpu_get_movable(self._h, p))
         return out[:self.lnv]
 
     def movable_from_batch(self, delete=None, insert=None):
@@ -319,54 +369,49 @@ class LouvainGPU:
         _ck(lib().mvgpu_get_converged(self._h, ctypes.byref(v)))
         return bool(v.value)
 
+    def _assignment(self, comm, refuse, rep):
+        """comm as the collective entry points take it: None, or an _Input of lnv ids.  A wrong shape still enters the
+        collective through `refuse`, flagged, so that the other ranks fail with this one instead of waiting for it."""
+        if comm is None:
+            return None
+        a = _Input(comm, "i8")
+        if a.ndim != 1 or a.size != self.lnv:
+            why = f"assignment has {a.size} entries, the shard has lnv = {self.lnv}"
+            _ck(refuse(self._h, why.encode(), ctypes.byref(rep)))
+            raise AssertionError("unreachable: a refused call fails")
+        return a
+
     def evaluate(self, comm=None):
         """Modularity Q and community counts of an assignment (lnv global community ids in [0, nv), caller's vertex
-        numbering, the form set_initial_communities takes); None evaluates what the last louvain() returned.  Collective:
-        every rank passes an array or every rank None; a bad id or an array whose length is not lnv on any rank raises
-        MvgpuError on every rank.  Returns mvgpu_quality as a dict (DESIGN.md §3.10)."""
+        numbering, the form set_initial_communities takes; a NumPy array or a torch tensor); None evaluates what the last
+        louvain() returned.  Collective: every rank passes an array or every rank None; a bad id or an array whose length
+        is not lnv on any rank raises MvgpuError on every rank.  Returns mvgpu_quality as a dict (DESIGN.md §3.10)."""
         q = Quality()
-        if comm is None:
-            _ck(lib().mvgpu_evaluate_communities(self._h, None, ctypes.byref(q)))
-            return q.as_dict()
-        comm = np.ascontiguousarray(comm, dtype=np.int64)
-        if comm.ndim != 1 or comm.size != self.lnv:
-            # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
-            why = f"assignment has {comm.size} entries, the shard has lnv = {self.lnv}"
-            _ck(lib().mv_evaluate_refused(self._h, why.encode(), ctypes.byref(q)))
-            raise AssertionError("unreachable: a refused evaluation fails")
-        buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
-        _ck(lib().mvgpu_evaluate_communities(self._h, buf.ctypes.data, ctypes.byref(q)))
+        a = self._assignment(comm, lib().mv_evaluate_refused, q)
+        _ck(lib().mvgpu_evaluate_communities(self._h, a and a.ptr, ctypes.byref(q)))
         return q.as_dict()
 
-    def split_communities(self, comm=None):
+    def split_communities(self, comm=None, device=False):
         """Split every community of an assignment into its connected pieces (DESIGN.md §3.12): Y gives each vertex the
         smallest global id of its component, where two vertices are joined when they share a community and the shard
         stores a record between them.  `comm` takes the form evaluate() takes; None splits what the last louvain()
         returned.  Collective, with evaluate()'s error rules.  Returns (Y, report): Y is this rank's lnv entries (int64,
-        a valid input to set_initial_communities and evaluate), report the global counts of mvgpu_split_report as a dict."""
+        a valid input to set_initial_communities and evaluate; a torch tensor on the context's device with device=True),
+        report the global counts of mvgpu_split_report as a dict."""
         rep = SplitReport()
-        out = np.zeros(max(self.lnv, 1), np.int64)
-        if comm is None:
-            _ck(lib().mvgpu_split_communities(self._h, None, out.ctypes.data, ctypes.byref(rep)))
-            return out[:self.lnv], rep.as_dict()
-        comm = np.ascontiguousarray(comm, dtype=np.int64)
-        if comm.ndim != 1 or comm.size != self.lnv:
-            # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
-            why = f"assignment has {comm.size} entries, the shard has lnv = {self.lnv}"
-            _ck(lib().mv_split_refused(self._h, why.encode(), ctypes.byref(rep)))
-            raise AssertionError("unreachable: a refused split fails")
-        buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
-        _ck(lib().mvgpu_split_communities(self._h, buf.ctypes.data, out.ctypes.data, ctypes.byref(rep)))
+        a = self._assignment(comm, lib().mv_split_refused, rep)
+        (out,), (p,) = _outputs(device, self.device, self.lnv, ("i8",))
+        _ck(lib().mvgpu_split_communities(self._h, a and a.ptr, p, ctypes.byref(rep)))
         return out[:self.lnv], rep.as_dict()
 
     def compare_communities(self, y, x=None):
         """Compare two assignments (DESIGN.md §3.13): contingency counts, pair counts, ARI, Rand index, NMI, VI and the
-        entropies, exact and the same on every rank count.  `y` and `x` take the form evaluate() takes; x = None compares
-        what the last louvain() returned.  Collective: every rank passes x or every rank None; a bad id or a wrong
-        length on any rank raises MvgpuError on every rank.  Returns mvgpu_compare_report as a dict; community_matches()
-        then gives the best match of every community of x."""
+        entropies, exact and the same on every rank count.  `y` and `x` take the form evaluate() takes (each a NumPy array
+        or a torch tensor, of either kind); x = None compares what the last louvain() returned.  Collective: every rank
+        passes x or every rank None; a bad id or a wrong length on any rank raises MvgpuError on every rank.  Returns
+        mvgpu_compare_report as a dict; community_matches() then gives the best match of every community of x."""
         rep = CompareReport()
-        arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.int64) for a in (x, y)]
+        arrs = [None if a is None else _Input(a, "i8") for a in (x, y)]
         bad = [a for a in arrs if a is not None and (a.ndim != 1 or a.size != self.lnv)]
         if y is None or bad:
             # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
@@ -374,59 +419,53 @@ class LouvainGPU:
                    f"assignment has {bad[0].size} entries, the shard has lnv = {self.lnv}")
             _ck(lib().mv_compare_refused(self._h, why.encode(), ctypes.byref(rep)))
             raise AssertionError("unreachable: a refused comparison fails")
-        bufs = [None if a is None else (a if a.size else np.zeros(1, np.int64)) for a in arrs]   # never NULL for an array
-        _ck(lib().mvgpu_compare_communities(self._h, None if bufs[0] is None else bufs[0].ctypes.data, bufs[1].ctypes.data,
-                                            ctypes.byref(rep)))
+        _ck(lib().mvgpu_compare_communities(self._h, arrs[0] and arrs[0].ptr, arrs[1].ptr, ctypes.byref(rep)))
         return rep.as_dict()
 
-    def probe(self, comm=None):
+    def probe(self, comm=None, device=False):
         """What every vertex would do under the Louvain rule from an assignment (DESIGN.md §3.15), without moving anything.
         `comm` takes the form evaluate() takes; None probes what the last louvain() returned.  Collective, with
         evaluate()'s error rules.  Returns (report, target, best, gain): mvgpu_probe_report as a dict (global counts), and
         this rank's lnv entries of the decision (int64), the best candidate community (int64, -1 without one) and its
-        gain (float64, -inf without one)."""
+        gain (float64, -inf without one); torch tensors on the context's device with device=True."""
         rep = ProbeReport()
-        n = max(self.lnv, 1)
-        target, best, gain = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(n, np.float64)
-        outs = (target.ctypes.data, best.ctypes.data, gain.ctypes.data)
-        if comm is None:
-            _ck(lib().mvgpu_probe_communities(self._h, None, *outs, ctypes.byref(rep)))
-        else:
-            comm = np.ascontiguousarray(comm, dtype=np.int64)
-            if comm.ndim != 1 or comm.size != self.lnv:
-                # still enter the collective, flagged, so that the other ranks fail with this one instead of waiting for it
-                why = f"assignment has {comm.size} entries, the shard has lnv = {self.lnv}"
-                _ck(lib().mv_probe_refused(self._h, why.encode(), ctypes.byref(rep)))
-                raise AssertionError("unreachable: a refused probe fails")
-            buf = comm if comm.size else np.zeros(1, np.int64)      # an empty shard still passes a non-NULL array
-            _ck(lib().mvgpu_probe_communities(self._h, buf.ctypes.data, *outs, ctypes.byref(rep)))
+        a = self._assignment(comm, lib().mv_probe_refused, rep)
+        (target, best, gain), outs = _outputs(device, self.device, self.lnv, ("i8", "i8", "f8"))
+        _ck(lib().mvgpu_probe_communities(self._h, a and a.ptr, *outs, ctypes.byref(rep)))
         return rep.as_dict(), target[:self.lnv], best[:self.lnv], gain[:self.lnv]
 
-    def community_matches(self):
+    def community_matches(self, device=False):
         """Per community of x in the last compare_communities(): entry s describes community parts[rank] + s.  Returns a
-        dict of int64 arrays `size`, `best`, `overlap` and `best_size`, lnv entries each (best = -1 for an empty x)."""
-        n = max(self.lnv, 1)
-        out = {k: np.zeros(n, np.int64) for k in ("size", "best", "overlap", "best_size")}
-        _ck(lib().mvgpu_get_community_matches(self._h, *[a.ctypes.data for a in out.values()]))
-        return {k: a[:self.lnv] for k, a in out.items()}
+        dict of int64 arrays `size`, `best`, `overlap` and `best_size`, lnv entries each (best = -1 for an empty x);
+        torch tensors on the context's device with device=True."""
+        names = ("size", "best", "overlap", "best_size")
+        out, ptrs = _outputs(device, self.device, self.lnv, ("i8",) * 4)
+        _ck(lib().mvgpu_get_community_matches(self._h, *ptrs))
+        return {k: a[:self.lnv] for k, a in zip(names, out)}
 
-    def community_stats(self):
+    def community_stats(self, device=False):
         """Per community of the last evaluate(): entry s describes community parts[rank] + s.  Returns a dict of
-        `size` (int64), `volume` and `internal` (float64), lnv entries each."""
-        n = max(self.lnv, 1)
-        size, vol, internal = np.zeros(n, np.int64), np.zeros(n, np.float64), np.zeros(n, np.float64)
-        _ck(lib().mvgpu_get_community_stats(self._h, size.ctypes.data, vol.ctypes.data, internal.ctypes.data))
+        `size` (int64), `volume` and `internal` (float64), lnv entries each; torch tensors on the context's device with
+        device=True."""
+        (size, vol, internal), ptrs = _outputs(device, self.device, self.lnv, ("i8", "f8", "f8"))
+        _ck(lib().mvgpu_get_community_stats(self._h, *ptrs))
         return {"size": size[:self.lnv], "volume": vol[:self.lnv], "internal": internal[:self.lnv]}
 
-    def compact_communities(self):
-        """Per vertex of the last evaluate(): its community's rank among the non-empty ids in ascending id (int64)."""
-        out = np.zeros(max(self.lnv, 1), np.int64)
-        _ck(lib().mvgpu_get_compact_communities(self._h, out.ctypes.data))
+    def compact_communities(self, device=False):
+        """Per vertex of the last evaluate(): its community's rank among the non-empty ids in ascending id (int64); a
+        torch tensor on the context's device with device=True."""
+        (out,), (p,) = _outputs(device, self.device, self.lnv, ("i8",))
+        _ck(lib().mvgpu_get_compact_communities(self._h, p))
         return out[:self.lnv]
 
-    def communities(self, out=None):
+    def communities(self, out=None, device=False):
         """currComm of this rank's vertices (global community ids).  `out`: optional preallocated int64 array
-        (a pinned one is filled at full PCIe rate)."""
+        (a pinned one is filled at full PCIe rate).  device=True: a torch tensor on the context's device instead."""
+        if device:
+            assert out is None, "device=True allocates its own tensor"
+            (t,), (p,) = _outputs(True, self.device, self.lnv, ("i8",))
+            _ck(lib().mvgpu_get_communities(self._h, p))
+            return t[:self.lnv]
         if out is None:
             out = np.empty(self.lnv, dtype=np.int64)
         assert out.dtype == np.int64 and out.size >= self.lnv and out.flags["C_CONTIGUOUS"]
