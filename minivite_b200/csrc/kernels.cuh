@@ -529,48 +529,66 @@ __global__ void __launch_bounds__(kTileV) k_scan_ws(const ScanParams p, const ui
   flush_acc<UNIT, TRACE, kTileV / 32>(p, acc_le_u, acc_le_d, acc_moved, acc_hash);
 }
 
+// The open-addressing table of heavy vertex p.heavy_list[blockIdx.x], built by its CTA (k_scan_heavy below,
+// k_probe_heavy in probe_gpu.cuh): 2x degree entries, a power of two, in HBM scratch, keyed by neighbour community.
+// Weighted sums are accumulated with fp64 atomics (order not fixed: weighted parity is tolerance-based anyway).
+template <bool UNIT>
+struct HeavyTable {
+  int32_t *keys;                 // neighbour community, -1: empty
+  int32_t *vi;                   // UNIT: edges into it
+  double *vd;                    // weighted: weight into it
+  unsigned int T;
+  __device__ __forceinline__ explicit HeavyTable(const ScanParams &p) {
+    const unsigned long long off = p.heavy_off[blockIdx.x];
+    T = (unsigned int)(p.heavy_off[blockIdx.x + 1] - off);
+    keys = p.hkeys + off;
+    vi = UNIT ? p.hvals_i + off : nullptr;
+    vd = UNIT ? nullptr : p.hvals_d + off;
+  }
+  __device__ __forceinline__ double val(unsigned int i) const { return UNIT ? (double)vi[i] : vd[i]; }
+  // clear the table, insert the edges [e0, e1), and leave the weight towards the own community cc (counter[0]) in w0
+  __device__ __forceinline__ void fill(const ScanParams &p, uint32_t e0, uint32_t e1, int cc, double &w0) const {
+    const int tid = threadIdx.x;
+    for (unsigned int i = tid; i < T; i += blockDim.x) { keys[i] = -1; if (UNIT) vi[i] = 0; else vd[i] = 0.0; }
+    __syncthreads();
+    for (uint32_t e = e0 + tid; e < e1; e += blockDim.x) {
+      const int c = __ldg(p.cur + p.tails[e]);
+      unsigned int h = (unsigned int)mix64((unsigned long long)c) & (T - 1);
+      for (;;) {
+        const int old = atomicCAS(&keys[h], -1, c);
+        if (old == -1 || old == c) {
+          if (UNIT) atomicAdd(&vi[h], 1); else atomicAdd(&vd[h], p.weights[e]);
+          break;
+        }
+        h = (h + 1) & (T - 1);
+      }
+    }
+    __syncthreads();
+    if (tid == 0) w0 = 0.0;
+    __syncthreads();
+    for (unsigned int i = tid; i < T; i += blockDim.x)
+      if (keys[i] == cc) w0 = val(i);
+    __syncthreads();
+  }
+};
+
 // ----------------------------------------------------------------------------------------------
-// High-degree vertices (degree > heavy_deg): one CTA per vertex, open-addressing table in HBM
-// scratch (2x degree entries) keyed by neighbour community; same decision rule.  Weighted sums are
-// accumulated with fp64 atomics here (order not fixed: weighted parity is tolerance-based anyway).
+// High-degree vertices (degree > heavy_deg): one CTA per vertex, its HeavyTable; same decision rule.
 // MASKED: a vertex with movable[v] == 0 still adds its counter[0] share and writes target = current.
 // ----------------------------------------------------------------------------------------------
 template <bool UNIT, bool MULTI, bool TRACE, bool MASKED = false>
 __global__ void __launch_bounds__(256) k_scan_heavy(const ScanParams p, const uint8_t *movable) {
   const int v = p.heavy_list[blockIdx.x];
-  const unsigned long long off = p.heavy_off[blockIdx.x];
-  const unsigned int T = (unsigned int)(p.heavy_off[blockIdx.x + 1] - off);   // power of two
-  int32_t *keys = p.hkeys + off;
-  int32_t *vi = UNIT ? p.hvals_i + off : nullptr;
-  double *vd = UNIT ? nullptr : p.hvals_d + off;
+  const HeavyTable<UNIT> tab(p);
   const int tid = threadIdx.x;
   const uint32_t e0 = p.rowptr[v], e1 = p.rowptr[v + 1];
   const int cc = p.cur[v];
-  for (unsigned int i = tid; i < T; i += blockDim.x) { keys[i] = -1; if (UNIT) vi[i] = 0; else vd[i] = 0.0; }
-  __syncthreads();
-  for (uint32_t e = e0 + tid; e < e1; e += blockDim.x) {
-    const int c = __ldg(p.cur + p.tails[e]);
-    unsigned int h = (unsigned int)mix64((unsigned long long)c) & (T - 1);
-    for (;;) {
-      const int old = atomicCAS(&keys[h], -1, c);
-      if (old == -1 || old == c) {
-        if (UNIT) atomicAdd(&vi[h], 1); else atomicAdd(&vd[h], p.weights[e]);
-        break;
-      }
-      h = (h + 1) & (T - 1);
-    }
-  }
-  __syncthreads();
   __shared__ double s_w0;
+  tab.fill(p, e0, e1, cc, s_w0);
   __shared__ double s_g[8];
   __shared__ int s_y[8];
   __shared__ long long s_sz[8];
   __shared__ int s_l[8];
-  if (tid == 0) s_w0 = 0.0;
-  __syncthreads();
-  for (unsigned int i = tid; i < T; i += blockDim.x)
-    if (keys[i] == cc) s_w0 = UNIT ? (double)vi[i] : vd[i];
-  __syncthreads();
   int owner; long long idx;
   locate_impl<MULTI>(p.pt, p.base, p.lnv, cc, owner, idx);
   double cc_deg, vdeg, sl; long long cc_size;
@@ -589,19 +607,20 @@ __global__ void __launch_bounds__(256) k_scan_heavy(const ScanParams p, const ui
   const double eix = __dsub_rn(w0, sl), ax = __dsub_rn(cc_deg, vdeg);
   double bg = 0.0; int by = cc; long long bsz = cc_size;
   int lby = kNoLabel;
-  for (unsigned int i = tid; i < T; i += blockDim.x) {
-    const int y = keys[i];
+  for (unsigned int i = tid; i < tab.T; i += blockDim.x) {
+    const int y = tab.keys[i];
     if (y < 0 || y == cc) continue;
     int yo; long long yi;
     locate_impl<MULTI>(p.pt, p.base, p.lnv, y, yo, yi);
-    double ay, eiy; long long ysz;
+    double ay; long long ysz;
     if (UNIT) {
       ysz = (long long)__ldg(ptr_csize<MULTI>(p, yo) + yi);
-      ay = (double)__ldg(ptr_cdeg<MULTI>(p, yo) + yi); eiy = (double)vi[i];
+      ay = (double)__ldg(ptr_cdeg<MULTI>(p, yo) + yi);
     } else {
       const CommW cw = ptr_cinfo_w<MULTI>(p, yo)[yi];
-      ysz = cw.size; ay = cw.degree; eiy = vd[i];
+      ysz = cw.size; ay = cw.degree;
     }
+    const double eiy = tab.val(i);
     const double g = gain_of(eiy, eix, vdeg, ay, ax, p.constant, p.f32);
     if (better_l<MULTI>(p, g, y, bg, by, lby)) { bg = g; by = y; bsz = ysz; }
   }

@@ -10,7 +10,8 @@
 // and four global counters: moves (target != X), vetoed (gain > 0 but held by the veto), interior (records, no
 // candidate) and the largest gain as an order-preserving key.
 // k_probe is k_scan_ws's tile layout around the shared per-vertex helpers of kernels.cuh (vertex_load, pass0, pass1 with
-// MARGIN, singleton_veto); k_probe_heavy is k_scan_heavy's hash-table reduction for vertices above heavy_deg.
+// MARGIN, singleton_veto); k_probe_heavy takes the vertices above heavy_deg on k_scan_heavy's hash table (HeavyTable,
+// kernels.cuh) with its own argmax.
 #pragma once
 #include "kernels.cuh"
 
@@ -140,55 +141,30 @@ __global__ void __launch_bounds__(kTileV) k_probe(const ScanParams p, const Prob
   probe_flush(o, n);
 }
 
-// one CTA per vertex above heavy_deg: k_scan_heavy's open-addressing table (2x degree entries, power of two, in HBM
-// scratch) keyed by neighbour community, then a CTA-wide argmax that starts at -inf and sends equal gains of any value
-// to the smaller id.  Weighted sums are added with fp64 atomics in any order, as in k_scan_heavy.
+// one CTA per vertex above heavy_deg: its HeavyTable (kernels.cuh), then a CTA-wide argmax that starts at -inf and
+// sends equal gains of any value to the smaller id.
 template <bool UNIT, bool MULTI>
 __global__ void __launch_bounds__(256) k_probe_heavy(const ScanParams p, const ProbeOut o) {
   const int v = p.heavy_list[blockIdx.x];
-  const unsigned long long off = p.heavy_off[blockIdx.x];
-  const unsigned int T = (unsigned int)(p.heavy_off[blockIdx.x + 1] - off);
-  int32_t *keys = p.hkeys + off;
-  int32_t *vi = UNIT ? p.hvals_i + off : nullptr;
-  double *vd = UNIT ? nullptr : p.hvals_d + off;
+  const HeavyTable<UNIT> tab(p);
   const int tid = threadIdx.x;
   const uint32_t e0 = p.rowptr[v], e1 = p.rowptr[v + 1];
   const int d = (int)(e1 - e0);
   const int cc = p.cur[v];
-  for (unsigned int i = tid; i < T; i += blockDim.x) { keys[i] = -1; if (UNIT) vi[i] = 0; else vd[i] = 0.0; }
-  __syncthreads();
-  for (uint32_t e = e0 + tid; e < e1; e += blockDim.x) {
-    const int c = __ldg(p.cur + p.tails[e]);
-    unsigned int h = (unsigned int)mix64((unsigned long long)c) & (T - 1);
-    for (;;) {
-      const int old = atomicCAS(&keys[h], -1, c);
-      if (old == -1 || old == c) {
-        if (UNIT) atomicAdd(&vi[h], 1); else atomicAdd(&vd[h], p.weights[e]);
-        break;
-      }
-      h = (h + 1) & (T - 1);
-    }
-  }
-  __syncthreads();
   __shared__ double s_w0;
+  tab.fill(p, e0, e1, cc, s_w0);
   __shared__ double s_g[8];
   __shared__ int s_y[8], s_l[8];
-  if (tid == 0) s_w0 = 0.0;
-  __syncthreads();
-  for (unsigned int i = tid; i < T; i += blockDim.x)
-    if (keys[i] == cc) s_w0 = UNIT ? (double)vi[i] : vd[i];
-  __syncthreads();
   double cc_deg, vdeg, sl;
   vertex_load<UNIT, MULTI>(p, v, cc, d, cc_deg, vdeg, sl);
   const double eix = __dsub_rn(s_w0, sl), ax = __dsub_rn(cc_deg, vdeg);
   double bg = -INFINITY;
   int by = -1, lby = kNoLabel;
-  for (unsigned int i = tid; i < T; i += blockDim.x) {
-    const int y = keys[i];
+  for (unsigned int i = tid; i < tab.T; i += blockDim.x) {
+    const int y = tab.keys[i];
     if (y < 0 || y == cc) continue;
-    double ay, eiy;
-    if (UNIT) { ay = (double)__ldg(at_cdeg<MULTI>(p, y)); eiy = (double)vi[i]; }
-    else { ay = __ldg(&at_cinfo_w<MULTI>(p, y)->degree); eiy = vd[i]; }
+    const double ay = UNIT ? (double)__ldg(at_cdeg<MULTI>(p, y)) : __ldg(&at_cinfo_w<MULTI>(p, y)->degree);
+    const double eiy = tab.val(i);
     const double g = gain_of(eiy, eix, vdeg, ay, ax, p.constant, p.f32);
     if (better_l<MULTI, true>(p, g, y, bg, by, lby)) { bg = g; by = y; }
   }

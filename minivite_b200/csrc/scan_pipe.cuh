@@ -78,6 +78,90 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---- the per-warp group pipeline of the persistent scan kernels, k_scan_pw below and k_scan_pq (scan_queue.cuh)
+// Each kernel carves its own shared memory and hands the pipeline NT tail buffers of PwCap<UNIT> edges (k_scan_pw 2,
+// k_scan_pq 1; weights beside them when !UNIT), 3 row-offset slots of kPwRows, and NT + 3 mbarriers at bar0: the tail
+// buffers' at [0, NT), the row slots' at [NT, NT + 3).  Lane 0 issues the copies.  The state carried from group to
+// group (ring positions, phase bits, what a tail buffer holds) stays with the kernel.
+template <bool UNIT, int NT>
+struct PwRing {
+  static constexpr int CAP = PwCap<UNIT>::value;
+  int32_t *s_c;                  // tails, then communities: [NT][CAP]
+  double *s_wt;                  // weights [NT][CAP], read when !UNIT
+  uint32_t *s_rows;              // row offsets [3][kPwRows]
+  uint32_t bar0;
+  int lane;
+
+  __device__ __forceinline__ void init() const {
+    if (lane == 0) {
+#pragma unroll
+      for (int b = 0; b < NT + 3; b++) mbar_init(bar0 + 8 * b, 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+  }
+  // row offsets rowptr[32*gg .. 32*gg + 36) -> ring slot
+  __device__ __forceinline__ void issue_rows(const ScanParams &p, int gg, int slot) const {
+    if (lane == 0) {
+      mbar_expect_tx(bar0 + 8 * (NT + slot), 36 * 4);
+      bulk_g2s(smem_u32(s_rows + slot * kPwRows), p.rowptr + (size_t)gg * 32, 36 * 4, bar0 + 8 * (NT + slot));
+    }
+  }
+  // edges [lo4, lo4 + n4), both multiples of 4, n4 <= CAP -> tail buffer b
+  __device__ __forceinline__ void issue_tails(const ScanParams &p, int b, uint32_t lo4, uint32_t n4) const {
+    if (lane == 0) {
+      mbar_expect_tx(bar0 + 8 * b, n4 * (UNIT ? 4u : 12u));
+      bulk_g2s(smem_u32(s_c + b * CAP), p.tails + lo4, n4 * 4u, bar0 + 8 * b);
+      if (!UNIT) bulk_g2s(smem_u32(s_wt + b * CAP), p.weights + lo4, n4 * 8u, bar0 + 8 * b);
+    }
+  }
+  // phase_bits: bit b = parity the next wait on barrier b expects
+  __device__ __forceinline__ void wait_bar(uint32_t &phase_bits, int b) const {
+    mbar_wait(bar0 + 8 * b, (phase_bits >> b) & 1u);
+    phase_bits ^= (1u << b);
+  }
+  // extent of a group's edge block from its (arrived) row offsets: [lo4, lo4 + n4), clipped to one buffer
+  __device__ __forceinline__ void extent(const ScanParams &p, int gg, int slot, uint32_t &lo4, uint32_t &n4) const {
+    const int nv = min(32, p.lnv - gg * 32);
+    const uint32_t e0 = s_rows[slot * kPwRows], e1 = s_rows[slot * kPwRows + nv];
+    lo4 = e0 & ~3u;
+    n4 = (e1 > lo4) ? min((uint32_t)CAP, (e1 - lo4 + 3u) & ~3u) : 0u;
+  }
+  // prologue: rows of the warp's first two groups into slots 0 and 1, tails of the first into buffer 0
+  __device__ __forceinline__ void prologue(const ScanParams &p, int g, int gstride, int ngroups, uint32_t &phase_bits,
+                                           uint32_t &have_lo, uint32_t &have_n) const {
+    if (g < ngroups) {
+      issue_rows(p, g, 0);
+      if (g + gstride < ngroups) issue_rows(p, g + gstride, 1);
+      wait_bar(phase_bits, NT);
+      extent(p, g, 0, have_lo, have_n);
+      if (have_n) issue_tails(p, 0, have_lo, have_n);
+    }
+  }
+  // the sub-range of a group that starts at lane `start` (ra, rb: this lane's row offsets, nvalid the group's size):
+  // the longest run [start, end) of non-heavy vertices whose edges [e_lo, e_end) fit one buffer.  Tail buffer b, which
+  // holds edges [have_lo, have_lo + have_n), is reloaded synchronously when it does not cover them (oversize group).
+  // False when the start vertex is heavy: the caller steps over it, k_scan_heavy takes it.
+  __device__ __forceinline__ bool sub_range(const ScanParams &p, int b, int start, int nvalid, uint32_t ra, uint32_t rb,
+                                            bool is_heavy, int &end, uint32_t &e_lo, uint32_t &e_end, uint32_t &have_lo,
+                                            uint32_t &have_n, uint32_t &phase_bits) const {
+    const uint32_t heavy_mask = __ballot_sync(0xffffffffu, is_heavy);
+    if ((heavy_mask >> start) & 1u) return false;
+    e_lo = __shfl_sync(0xffffffffu, ra, start);
+    const uint32_t a_sub = e_lo & ~3u;
+    const bool fits = lane >= start && lane < nvalid && !is_heavy && (rb - a_sub) <= (uint32_t)CAP;
+    const uint32_t stop_mask = ~__ballot_sync(0xffffffffu, fits) & (0xffffffffu << start);
+    end = stop_mask ? (__ffs(stop_mask) - 1) : 32;               // > start: the start vertex always fits
+    e_end = __shfl_sync(0xffffffffu, rb, end - 1);
+    if (!(a_sub >= have_lo && e_end <= have_lo + have_n)) {
+      have_lo = a_sub;
+      have_n = (e_end - a_sub + 3u) & ~3u;
+      if (have_n) { issue_tails(p, b, have_lo, have_n); wait_bar(phase_bits, b); }
+    }
+    return true;
+  }
+};
+
 // MASKED (DESIGN.md §3.14): a vertex with movable[v] == 0 skips pass 1 and stays (counter[0] still counted).
 template <bool UNIT, bool MULTI, bool TRACE, bool FIRST, bool MASKED = false>
 __global__ void __launch_bounds__(kPwWarps * 32, UNIT ? MV_PW_RES_WARPS / kPwWarps : 24 / kPwWarps)
@@ -91,82 +175,42 @@ k_scan_pw(const ScanParams p, int ngroups, const uint8_t *movable) {
   constexpr int kWarpBytes = PwWarpBytes<UNIT>::value;
   static_assert(CAP % 4 == 0 && kPwRows % 4 == 0, "buffers must be 16-byte multiples");
   unsigned char *wbase = smem_raw + (size_t)wid * kWarpBytes;
-  int32_t *s_c = reinterpret_cast<int32_t *>(wbase);
-  double *s_wt = reinterpret_cast<double *>(wbase + 2 * CAP * 4);
-  uint32_t *s_rows = reinterpret_cast<uint32_t *>(wbase + 2 * CAP * (UNIT ? 4 : 12));
-  const uint32_t bar0 = smem_u32(wbase + 2 * CAP * (UNIT ? 4 : 12) + 3 * kPwRows * 4);   // [0,1] tails, [2,3,4] rows
-
-  if (lane == 0) {
-#pragma unroll
-    for (int b = 0; b < 5; b++) mbar_init(bar0 + 8 * b, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
+  const PwRing<UNIT, 2> ring{reinterpret_cast<int32_t *>(wbase), reinterpret_cast<double *>(wbase + 2 * CAP * 4),
+                             reinterpret_cast<uint32_t *>(wbase + 2 * CAP * (UNIT ? 4 : 12)),
+                             smem_u32(wbase + 2 * CAP * (UNIT ? 4 : 12) + 3 * kPwRows * 4), lane};
+  ring.init();
   const int gstride = gridDim.x * kPwWarps;
   int g = blockIdx.x * kPwWarps + wid;
 
   unsigned long long acc_le_u = 0, acc_moved = 0, acc_hash = 0;
   double acc_le_d = 0.0;
-  uint32_t phase_bits = 0;                       // bit b = parity the next wait on barrier b expects
+  uint32_t phase_bits = 0;
 
-  // ---- producers (lane 0) and consumers of the two rings
-  auto issue_rows = [&](int gg, int slot) {      // row offsets rowptr[32*gg .. 32*gg + 36) -> ring slot
-    if (lane == 0) {
-      mbar_expect_tx(bar0 + 8 * (2 + slot), 36 * 4);
-      bulk_g2s(smem_u32(s_rows + slot * kPwRows), p.rowptr + (size_t)gg * 32, 36 * 4, bar0 + 8 * (2 + slot));
-    }
-  };
-  auto issue_tails = [&](int b, uint32_t lo4, uint32_t n4) {   // edges [lo4, lo4 + n4), both multiples of 4, n4 <= CAP
-    if (lane == 0) {
-      mbar_expect_tx(bar0 + 8 * b, n4 * (UNIT ? 4u : 12u));
-      bulk_g2s(smem_u32(s_c + b * CAP), p.tails + lo4, n4 * 4u, bar0 + 8 * b);
-      if (!UNIT) bulk_g2s(smem_u32(s_wt + b * CAP), p.weights + lo4, n4 * 8u, bar0 + 8 * b);
-    }
-  };
-  auto wait_bar = [&](int b) {
-    mbar_wait(bar0 + 8 * b, (phase_bits >> b) & 1u);
-    phase_bits ^= (1u << b);
-  };
-  // extent of a group's edge block from its (arrived) row offsets: [lo4, lo4 + n4), clipped to one buffer
-  auto extent = [&](int gg, int slot, uint32_t &lo4, uint32_t &n4) {
-    const int nv = min(32, p.lnv - gg * 32);
-    const uint32_t e0 = s_rows[slot * kPwRows], e1 = s_rows[slot * kPwRows + nv];
-    lo4 = e0 & ~3u;
-    n4 = (e1 > lo4) ? min((uint32_t)CAP, (e1 - lo4 + 3u) & ~3u) : 0u;
-  };
-
-  // ---- prologue: rows of the first two groups, tails of the first
   int rslot = 0, buf = 0;                        // ring positions of the current group
   uint32_t have_lo = 0, have_n = 0;              // what the current tail buffer holds: edges [have_lo, have_lo + have_n)
-  if (g < ngroups) {
-    issue_rows(g, 0);
-    if (g + gstride < ngroups) issue_rows(g + gstride, 1);
-    wait_bar(2);
-    extent(g, 0, have_lo, have_n);
-    if (have_n) issue_tails(0, have_lo, have_n);
-  }
+  ring.prologue(p, g, gstride, ngroups, phase_bits, have_lo, have_n);
 
   for (; g < ngroups; g += gstride) {
     // ---- keep the rings full: rows of group k+2, tails of group k+1 (its rows arrived one iteration ago)
     const int rs1 = rslot == 2 ? 0 : rslot + 1, rs2 = rs1 == 2 ? 0 : rs1 + 1;
-    if (g + 2 * gstride < ngroups) issue_rows(g + 2 * gstride, rs2);
+    if (g + 2 * gstride < ngroups) ring.issue_rows(p, g + 2 * gstride, rs2);
     uint32_t nx_lo = 0, nx_n = 0;
     if (g + gstride < ngroups) {
-      wait_bar(2 + rs1);
-      extent(g + gstride, rs1, nx_lo, nx_n);
-      if (nx_n) issue_tails(buf ^ 1, nx_lo, nx_n);
+      ring.wait_bar(phase_bits, 2 + rs1);
+      ring.extent(p, g + gstride, rs1, nx_lo, nx_n);
+      if (nx_n) ring.issue_tails(p, buf ^ 1, nx_lo, nx_n);
     }
-    if (have_n) wait_bar(buf);
+    if (have_n) ring.wait_bar(phase_bits, buf);
 
     const int v = g * 32 + lane;
     const int nvalid = min(32, p.lnv - g * 32);
-    const uint32_t *rows = s_rows + rslot * kPwRows;
+    const uint32_t *rows = ring.s_rows + rslot * kPwRows;
     uint32_t ra = 0, rb = 0;
     if (lane < nvalid) { ra = rows[lane]; rb = rows[lane + 1]; }
     const uint32_t deg = rb - ra;
     const bool is_heavy = p.has_heavy && deg > (uint32_t)p.heavy_deg;
-    int32_t *sc = s_c + buf * CAP;
-    double *sw = s_wt + buf * CAP;
+    int32_t *sc = ring.s_c + buf * CAP;
+    double *sw = ring.s_wt + buf * CAP;
     const uint32_t g_e0 = rows[0], g_e1 = rows[nvalid];
     // the common case: no vertex of the shard is heavy and the whole group sits in the prefetched buffer
     const bool whole = !p.has_heavy && (g_e1 - have_lo) <= have_n;
@@ -176,21 +220,9 @@ k_scan_pw(const ScanParams p, int ngroups, const uint8_t *movable) {
       // ---- sub-range [start, end): longest run of non-heavy vertices whose edges fit the buffer
       int end = nvalid;
       uint32_t e_lo = g_e0, e_end = g_e1;
-      if (!whole) {
-        const uint32_t heavy_mask = __ballot_sync(0xffffffffu, is_heavy);
-        if ((heavy_mask >> start) & 1u) { start++; continue; }
-        e_lo = __shfl_sync(0xffffffffu, ra, start);
-        const uint32_t a_sub = e_lo & ~3u;
-        const bool fits = lane >= start && lane < nvalid && !is_heavy && (rb - a_sub) <= (uint32_t)CAP;
-        const uint32_t stop_mask = ~__ballot_sync(0xffffffffu, fits) & (0xffffffffu << start);
-        end = stop_mask ? (__ffs(stop_mask) - 1) : 32;               // > start: the start vertex always fits
-        e_end = __shfl_sync(0xffffffffu, rb, end - 1);
-        if (!(a_sub >= have_lo && e_end <= have_lo + have_n)) {
-          // not covered by what the buffer holds (oversize group): synchronous bulk copy of this sub-range
-          have_lo = a_sub;
-          have_n = (e_end - a_sub + 3u) & ~3u;
-          if (have_n) { issue_tails(buf, have_lo, have_n); wait_bar(buf); }
-        }
+      if (!whole && !ring.sub_range(p, buf, start, nvalid, ra, rb, is_heavy, end, e_lo, e_end, have_lo, have_n, phase_bits)) {
+        start++;
+        continue;
       }
       const bool mine = lane >= start && lane < end;
       const int d = mine ? (int)deg : 0;

@@ -15,9 +15,10 @@
 //     free, so ONE buffer suffices (the next group's bulk copy is issued right after pass 0): 6.5 KB of shared memory
 //     per warp against k_scan_pw's 4.8 KB.
 // A group that holds a hard vertex with more leftovers than a ring slot takes (early iterations: every neighbour is a
-// different community) runs pass 1 in place like k_scan_pw.  Everything else -- groups of 32 vertices per warp,
-// persistent grid, row offsets and tails through cp.async.bulk + mbarrier, 16-byte phase A, sub-ranges, heavy
-// vertices -- is k_scan_pw's (scan_pipe.cuh).
+// different community) runs pass 1 in place like k_scan_pw.  Groups of 32 vertices per warp, the persistent grid, the
+// row offsets and tails through cp.async.bulk + mbarrier, the sub-ranges and the heavy vertices come from the pipeline
+// it shares with k_scan_pw (PwRing, scan_pipe.cuh), here with one tail buffer.  The 16-byte phase A is k_scan_pw's,
+// written out again: as a shared helper it costs k_scan_pw registers and spills.
 #pragma once
 #include "scan_pipe.cuh"
 
@@ -51,17 +52,11 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
   // int4 [kQSlots] {vertex, community, m | degree << 16, community degree} | 4 mbarriers (tails, rows x3)
   unsigned char *wbase = smem_raw + (size_t)wid * kPqWarpBytes;
   int32_t *sc = reinterpret_cast<int32_t *>(wbase);
-  uint32_t *s_rows = reinterpret_cast<uint32_t *>(wbase + CAP * 4);
+  const PwRing<true, 1> ring{sc, nullptr, reinterpret_cast<uint32_t *>(wbase + CAP * 4),
+                             smem_u32(wbase + CAP * 4 + 3 * kPwRows * 4 + kQSlots * kQEnt * 4 + kQSlots * 16), lane};
   int32_t *q_ent = reinterpret_cast<int32_t *>(wbase + CAP * 4 + 3 * kPwRows * 4);
   int4 *q_hdr = reinterpret_cast<int4 *>(wbase + CAP * 4 + 3 * kPwRows * 4 + kQSlots * kQEnt * 4);
-  const uint32_t bar0 = smem_u32(wbase + CAP * 4 + 3 * kPwRows * 4 + kQSlots * kQEnt * 4 + kQSlots * 16);   // [0] tails, [1..3] rows
-
-  if (lane == 0) {
-#pragma unroll
-    for (int b = 0; b < 4; b++) mbar_init(bar0 + 8 * b, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
+  ring.init();
   const int gstride = gridDim.x * kPwWarps;
   int g = blockIdx.x * kPwWarps + wid;
 
@@ -69,28 +64,6 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
   uint32_t phase_bits = 0;
   int qhead = 0, qcount = 0;                     // ring state (warp-uniform)
 
-  auto issue_rows = [&](int gg, int slot) {
-    if (lane == 0) {
-      mbar_expect_tx(bar0 + 8 * (1 + slot), 36 * 4);
-      bulk_g2s(smem_u32(s_rows + slot * kPwRows), p.rowptr + (size_t)gg * 32, 36 * 4, bar0 + 8 * (1 + slot));
-    }
-  };
-  auto issue_tails = [&](uint32_t lo4, uint32_t n4) {
-    if (lane == 0) {
-      mbar_expect_tx(bar0, n4 * 4u);
-      bulk_g2s(smem_u32(sc), p.tails + lo4, n4 * 4u, bar0);
-    }
-  };
-  auto wait_bar = [&](int b) {
-    mbar_wait(bar0 + 8 * b, (phase_bits >> b) & 1u);
-    phase_bits ^= (1u << b);
-  };
-  auto extent = [&](int gg, int slot, uint32_t &lo4, uint32_t &n4) {
-    const int nv = min(32, p.lnv - gg * 32);
-    const uint32_t e0 = s_rows[slot * kPwRows], e1 = s_rows[slot * kPwRows + nv];
-    lo4 = e0 & ~3u;
-    n4 = (e1 > lo4) ? min((uint32_t)CAP, (e1 - lo4 + 3u) & ~3u) : 0u;
-  };
   // pass 1 + singleton veto (kernels.cuh) for one vertex whose leftover communities sit in seg[0..m).  All lanes call
   // it; lanes without work pass m = 0.  Returns the chosen community.
   // (The same bound per candidate -- skip the exact gain when fl(2 (c - e_ix) + gB) is below the best gain so far -- was
@@ -123,22 +96,16 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
 
   int rslot = 0;
   uint32_t have_lo = 0, have_n = 0;
-  if (g < ngroups) {
-    issue_rows(g, 0);
-    if (g + gstride < ngroups) issue_rows(g + gstride, 1);
-    wait_bar(1);
-    extent(g, 0, have_lo, have_n);
-    if (have_n) issue_tails(have_lo, have_n);
-  }
+  ring.prologue(p, g, gstride, ngroups, phase_bits, have_lo, have_n);
 
   for (; g < ngroups; g += gstride) {
     const int rs1 = rslot == 2 ? 0 : rslot + 1, rs2 = rs1 == 2 ? 0 : rs1 + 1;
-    if (g + 2 * gstride < ngroups) issue_rows(g + 2 * gstride, rs2);
-    if (have_n) wait_bar(0);
+    if (g + 2 * gstride < ngroups) ring.issue_rows(p, g + 2 * gstride, rs2);
+    if (have_n) ring.wait_bar(phase_bits, 0);
 
     const int v = g * 32 + lane;
     const int nvalid = min(32, p.lnv - g * 32);
-    const uint32_t *rows = s_rows + rslot * kPwRows;
+    const uint32_t *rows = ring.s_rows + rslot * kPwRows;
     uint32_t ra = 0, rb = 0;
     if (lane < nvalid) { ra = rows[lane]; rb = rows[lane + 1]; }
     const uint32_t deg = rb - ra;
@@ -150,20 +117,9 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
     while (start < nvalid) {
       int end = nvalid;
       uint32_t e_lo = g_e0, e_end = g_e1;
-      if (!whole) {
-        const uint32_t heavy_mask = __ballot_sync(0xffffffffu, is_heavy);
-        if ((heavy_mask >> start) & 1u) { start++; continue; }
-        e_lo = __shfl_sync(0xffffffffu, ra, start);
-        const uint32_t a_sub = e_lo & ~3u;
-        const bool fits = lane >= start && lane < nvalid && !is_heavy && (rb - a_sub) <= (uint32_t)CAP;
-        const uint32_t stop_mask = ~__ballot_sync(0xffffffffu, fits) & (0xffffffffu << start);
-        end = stop_mask ? (__ffs(stop_mask) - 1) : 32;
-        e_end = __shfl_sync(0xffffffffu, rb, end - 1);
-        if (!(a_sub >= have_lo && e_end <= have_lo + have_n)) {
-          have_lo = a_sub;
-          have_n = (e_end - a_sub + 3u) & ~3u;
-          if (have_n) { issue_tails(have_lo, have_n); wait_bar(0); }
-        }
+      if (!whole && !ring.sub_range(p, 0, start, nvalid, ra, rb, is_heavy, end, e_lo, e_end, have_lo, have_n, phase_bits)) {
+        start++;
+        continue;
       }
       const bool mine = lane >= start && lane < end;
       const int d = mine ? (int)deg : 0;
@@ -248,9 +204,9 @@ __global__ void __launch_bounds__(kPwWarps * 32, MV_PW_RES_WARPS / kPwWarps) k_s
     // ---- the tail buffer is free: next group's tails (its rows arrived while this group was reduced)
     have_lo = 0; have_n = 0;
     if (g + gstride < ngroups) {
-      wait_bar(1 + rs1);
-      extent(g + gstride, rs1, have_lo, have_n);
-      if (have_n) issue_tails(have_lo, have_n);
+      ring.wait_bar(phase_bits, 1 + rs1);
+      ring.extent(p, g + gstride, rs1, have_lo, have_n);
+      if (have_n) ring.issue_tails(p, 0, have_lo, have_n);
     }
     // ---- enough hard vertices waiting: pass 1 with one vertex per lane while the copy is in flight
     while (qcount >= kQDrain) drain(min(qcount, 32));
