@@ -162,7 +162,8 @@ struct mvgpu_ctx {
   DevBuf<Edge16> raw_ring;             // compact upload: raw chunks narrowed on the device (two slots)
   long long raw_chunks = 0;
   DevBuf<long long> wide;              // int64 per-vertex arrays on their way to or from host memory
-  void *h_bounce[2] = {nullptr, nullptr};   // pinned chunks between wide and pageable host arrays, both ways
+  void *h_bounce[2] = {nullptr, nullptr};   // pinned chunks between the device and pageable host arrays, both ways
+  cudaEvent_t bounce_ev[2] = {nullptr, nullptr};   // the last copy in or out of h_bounce[b]
   DevBuf<unsigned long long> take_bad; // k_take_ids: the smallest local index of a bad id
   const int32_t *d_tails32 = nullptr;
   long long in_nremote = 0;
@@ -1380,29 +1381,73 @@ std::string locate(const mvgpu_ctx *c, const void *p, const char *name, Where &w
   return "";
 }
 
-constexpr long long kBounce = 4LL << 20;       // int64 entries per pinned bounce buffer (32 MB)
+// The one rule for moving a caller's bytes: device memory is used in place, pinned memory takes one copy, and pageable
+// memory goes through the two pinned bounce buffers in chunks (instead of the driver's staged pageable copy),
+// double-buffered in both directions (DESIGN.md §3.16).  bounce_ev[b] is recorded after every copy in or out of h_bounce[b], so
+// waiting on it makes the buffer free to refill, whichever routine used it last.
+constexpr size_t kBounce = 32u << 20;          // bytes per pinned bounce buffer
 
 int bounce_buffers(mvgpu_ctx *c) {
-  for (int b = 0; b < 2; b++)
-    if (!c->h_bounce[b]) CK(cudaMallocHost(&c->h_bounce[b], kBounce * sizeof(long long)));
+  for (int b = 0; b < 2; b++) {
+    if (!c->h_bounce[b]) CK(cudaMallocHost(&c->h_bounce[b], kBounce));
+    if (!c->bounce_ev[b]) CK(cudaEventCreateWithFlags(&c->bounce_ev[b], cudaEventDisableTiming));
+  }
   return 0;
 }
 
-// n int64 of pageable host memory -> c->wide, in chunks through the two pinned bounce buffers (full PCIe rate instead of
-// the driver's staged pageable path): the reverse of mvgpu_get_communities.  Asynchronous; the source may change once
-// this returns.
-int stage_pageable(mvgpu_ctx *c, const int64_t *src, long long n) {
+// `bytes` of the caller's array src (class w) as the device reads them: dev = src for device memory, else a copy in
+// staging (grown to fit).  Asynchronous on the context's stream: pageable memory may change once this returns, pinned
+// and device memory once the stream has passed the copy (every entry point synchronises before it returns).
+template <typename T>
+int to_device(mvgpu_ctx *c, const void *src, size_t bytes, Where w, DevBuf<T> &staging, const T *&dev) {
+  dev = static_cast<const T *>(src);
+  if (w == Where::Device) return 0;
+  TRY(staging.ensure((bytes + sizeof(T) - 1) / sizeof(T)));
+  dev = staging.p;
+  char *to = reinterpret_cast<char *>(staging.p);
+  if (w == Where::Pinned) {
+    CK(cudaMemcpyAsync(to, src, bytes, cudaMemcpyHostToDevice, c->stream));
+    return 0;
+  }
+  if (bytes == 0) return 0;
   TRY(bounce_buffers(c));
-  cudaEvent_t ev[2] = {get_event(c, 0), get_event(c, 1)};
-  long long off = 0;
-  for (int k = 0; off < n; k++) {
+  for (size_t off = 0, k = 0; off < bytes; k++) {
     const int b = k & 1;
-    const long long m = std::min(kBounce, n - off);
-    CK(cudaEventSynchronize(ev[b]));           // the copy out of this buffer two chunks ago (or in an earlier call) is done
-    memcpy(c->h_bounce[b], src + off, sizeof(long long) * m);
-    CK(cudaMemcpyAsync(c->wide.p + off, c->h_bounce[b], sizeof(long long) * m, cudaMemcpyHostToDevice, c->stream));
-    CK(cudaEventRecord(ev[b], c->stream));
+    const size_t m = std::min(kBounce, bytes - off);
+    CK(cudaEventSynchronize(c->bounce_ev[b]));
+    memcpy(c->h_bounce[b], static_cast<const char *>(src) + off, m);
+    CK(cudaMemcpyAsync(to + off, c->h_bounce[b], m, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaEventRecord(c->bounce_ev[b], c->stream));
     off += m;
+  }
+  return 0;
+}
+
+// `bytes` of device memory src -> the caller's array dst (class w).  Synchronous.
+int to_caller(mvgpu_ctx *c, const void *src, size_t bytes, Where w, void *dst) {
+  if (bytes == 0) return 0;
+  cudaStream_t s = c->stream;
+  if (w != Where::Pageable) {
+    CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s));
+    CK(cudaStreamSynchronize(s));
+    return 0;
+  }
+  TRY(bounce_buffers(c));
+  size_t at[2] = {0, 0}, pend[2] = {0, 0};     // per buffer: the chunk whose copy into it is in flight
+  for (size_t off = 0, k = 0; off < bytes || pend[0] || pend[1]; k++) {
+    const int b = k & 1;
+    if (pend[b]) {                             // drain this buffer while the other buffer's copy is in flight
+      CK(cudaEventSynchronize(c->bounce_ev[b]));
+      memcpy(static_cast<char *>(dst) + at[b], c->h_bounce[b], pend[b]);
+      pend[b] = 0;
+    }
+    if (off < bytes) {
+      const size_t m = std::min(kBounce, bytes - off);
+      CK(cudaMemcpyAsync(c->h_bounce[b], static_cast<const char *>(src) + off, m, cudaMemcpyDeviceToHost, s));
+      CK(cudaEventRecord(c->bounce_ev[b], s));
+      at[b] = off; pend[b] = m;
+      off += m;
+    }
   }
   return 0;
 }
@@ -1421,13 +1466,8 @@ int take_ids(mvgpu_ctx *c, const int64_t *ids, const char *who, const char *name
   const long long n = c->lnv;
   if (n == 0) return 0;
   cudaStream_t s = c->stream;
-  const long long *src = reinterpret_cast<const long long *>(ids);
-  if (w != Where::Device) {
-    TRY(c->wide.ensure(n));
-    if (w == Where::Pinned) CK(cudaMemcpyAsync(c->wide.p, ids, sizeof(long long) * n, cudaMemcpyHostToDevice, s));
-    else TRY(stage_pageable(c, ids, n));
-    src = c->wide.p;
-  }
+  const long long *src;
+  TRY(to_device(c, ids, sizeof(long long) * n, w, c->wide, src));
   TRY(c->take_bad.ensure(1));
   CK(cudaMemsetAsync(c->take_bad.p, 0xff, sizeof(unsigned long long), s));
   k_take_ids<<<grid_for(n, 256, c->num_sms), 256, 0, s>>>(src, n, c->nv_global, dst, c->take_bad.p);
@@ -1445,8 +1485,8 @@ int take_ids(mvgpu_ctx *c, const int64_t *ids, const char *who, const char *name
   return 0;
 }
 
-// lnv int32 ids on the device -> the caller's int64 array (class w): widened straight into device memory, through wide
-// and one copy into host memory.  Synchronous.
+// lnv int32 ids on the device -> the caller's int64 array (class w): widened straight into device memory, or into wide
+// and from there to host memory.  Synchronous.
 int put_ids(mvgpu_ctx *c, const int32_t *src, int64_t *out, Where w) {
   const long long n = c->lnv;
   if (n == 0) return 0;
@@ -1457,7 +1497,7 @@ int put_ids(mvgpu_ctx *c, const int32_t *src, int64_t *out, Where w) {
   }
   k_widen<<<grid_for(n, 256, c->num_sms), 256, 0, c->stream>>>(src, n, dst);
   CK(cudaGetLastError());
-  if (w != Where::Device) CK(cudaMemcpyAsync(out, c->wide.p, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
+  if (w != Where::Device) return to_caller(c, dst, sizeof(long long) * n, w, out);
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -1753,10 +1793,7 @@ int probe(mvgpu_ctx *c, const int64_t *comm, int64_t *target, int64_t *best, dou
   TRY(assignment_pass(c, ev, [&] { return probe_pass(c, r); }, r.probe_s));
   if (target) TRY(put_ids(c, c->probe_tgt.p, target, w[0]));
   if (best) TRY(put_ids(c, c->probe_best.p, best, w[1]));
-  if (gain && c->lnv > 0) {
-    CK(cudaMemcpyAsync(gain, c->probe_gain.p, sizeof(double) * c->lnv, cudaMemcpyDefault, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-  }
+  if (gain) TRY(to_caller(c, c->probe_gain.p, sizeof(double) * c->lnv, w[2], gain));
   *rep = r;
   return 0;
 }
@@ -2053,22 +2090,10 @@ int merge_records(mvgpu_ctx *c, long long n, const long long *rowptr, const Edge
   return 0;
 }
 
-// A batch array of n entries as the kernels read it: the caller's own when it is device memory (dev), else a copy in buf
-template <typename T>
-int batch_array(mvgpu_ctx *c, const T *p, long long n, bool dev, DevBuf<T> &buf, const T *&out) {
-  out = p;
-  if (dev) return 0;
-  TRY(buf.ensure(n));
-  if (n) CK(cudaMemcpyAsync(buf.p, p, sizeof(T) * n, cudaMemcpyHostToDevice, c->stream));
-  out = buf.p;
-  return 0;
-}
-
-// This rank's part of mvgpu_update_shard before the agreement: the batch to the device (dev[k]: array k, in the order of
-// the arguments, is device memory and is read in place), validated, sorted and merged into nrow / nedges.  Leaves the
-// shard itself as it is.
+// This rank's part of mvgpu_update_shard before the agreement: the batch to the device (wh[k]: the class of array k, in
+// the order of the arguments), validated, sorted and merged into nrow / nedges.  Leaves the shard itself as it is.
 int update_prepare(mvgpu_ctx *c, long long n_del, const int64_t *del_src, const int64_t *del_dst, long long n_ins,
-                   const int64_t *ins_src, const int64_t *ins_dst, const double *ins_weight, const bool *dev,
+                   const int64_t *ins_src, const int64_t *ins_dst, const double *ins_weight, const Where *wh,
                    DevBuf<long long> &nrow, DevBuf<Edge16> &nedges, long long *lne_out) {
   cudaStream_t s = c->stream;
   const int nsm = c->num_sms;
@@ -2081,11 +2106,11 @@ int update_prepare(mvgpu_ctx *c, long long n_del, const int64_t *del_src, const 
   TRY(iidx.ensure(n_ins)); TRY(iidx_s.ensure(n_ins)); TRY(bad.ensure(1));
   const long long *ds, *dd, *is, *id;
   const double *w;
-  TRY(batch_array(c, reinterpret_cast<const long long *>(del_src), n_del, dev[0], dsrc, ds));
-  TRY(batch_array(c, reinterpret_cast<const long long *>(del_dst), n_del, dev[1], ddst, dd));
-  TRY(batch_array(c, reinterpret_cast<const long long *>(ins_src), n_ins, dev[2], isrc, is));
-  TRY(batch_array(c, reinterpret_cast<const long long *>(ins_dst), n_ins, dev[3], idst, id));
-  TRY(batch_array(c, ins_weight, n_ins, dev[4], iw, w));
+  TRY(to_device(c, del_src, sizeof(long long) * n_del, wh[0], dsrc, ds));
+  TRY(to_device(c, del_dst, sizeof(long long) * n_del, wh[1], ddst, dd));
+  TRY(to_device(c, ins_src, sizeof(long long) * n_ins, wh[2], isrc, is));
+  TRY(to_device(c, ins_dst, sizeof(long long) * n_ins, wh[3], idst, id));
+  TRY(to_device(c, ins_weight, sizeof(double) * n_ins, wh[4], iw, w));
   CK(cudaMemsetAsync(bad.p, 0, sizeof(unsigned int), s));
   k_rowptr_check<<<grid_for(c->lnv + 1, 256, nsm), 256, 0, s>>>(c->d_rowptr64, c->lnv, c->lne, bad.p);
   if (n_del) k_batch_keys<<<grid_for(n_del, 256, nsm), 256, 0, s>>>(ds, dd, n_del, c->base, c->bound, c->nv_global, dkey.p, nullptr, bad.p);
@@ -2226,7 +2251,10 @@ int mvgpu_destroy(mvgpu_ctx *c) {
   c->hc.close_comm();
   for (cudaEvent_t e : c->events) cudaEventDestroy(e);
   if (c->h_stage) cudaFreeHost(c->h_stage);
-  for (int b = 0; b < 2; b++) if (c->h_bounce[b]) cudaFreeHost(c->h_bounce[b]);
+  for (int b = 0; b < 2; b++) {
+    if (c->h_bounce[b]) cudaFreeHost(c->h_bounce[b]);
+    if (c->bounce_ev[b]) cudaEventDestroy(c->bounce_ev[b]);
+  }
   if (c->h_pin) cudaFreeHost(c->h_pin);
   if (c->stream) cudaStreamDestroy(c->stream);
   delete c;                                    // the DevBufs free themselves
@@ -2551,20 +2579,18 @@ int mvgpu_update_shard(mvgpu_ctx *c, int64_t n_del, const int64_t *del_src, cons
   else if (n_del < 0 || n_ins < 0) err = "negative batch size";
   else if (n_del >= (1LL << 31) || n_ins >= (1LL << 31)) err = "batch too large: fewer than 2^31 deletions and 2^31 insertions per call";
   else if ((n_del && (!del_src || !del_dst)) || (n_ins && (!ins_src || !ins_dst || !ins_weight))) err = "null batch array";
-  bool dev[5] = {};
+  Where w[5];
   if (err.empty()) {                            // the arrays of an empty side are not read
     const void *arr[5] = {n_del ? del_src : nullptr, n_del ? del_dst : nullptr, n_ins ? ins_src : nullptr,
                           n_ins ? ins_dst : nullptr, n_ins ? ins_weight : nullptr};
     const char *names[5] = {"del_src", "del_dst", "ins_src", "ins_dst", "ins_weight"};
-    Where w[5];
     err = locate_all(c, 5, arr, names, w);
-    for (int k = 0; k < 5; k++) dev[k] = w[k] == Where::Device;
   }
   if (!err.empty()) err = "mvgpu_update_shard: " + err;
   DevBuf<long long> nrow;
   DevBuf<Edge16> nedges;
   long long lne2 = 0;
-  if (err.empty() && update_prepare(c, n_del, del_src, del_dst, n_ins, ins_src, ins_dst, ins_weight, dev, nrow, nedges, &lne2)) err = g_err;
+  if (err.empty() && update_prepare(c, n_del, del_src, del_dst, n_ins, ins_src, ins_dst, ins_weight, w, nrow, nedges, &lne2)) err = g_err;
   if (c->nranks > 1) {
     TRY(c->scratch.ensure(sizeof(Scalars)));
     long long any = err.empty() ? 0 : 1;
@@ -2624,11 +2650,8 @@ int mvgpu_set_movable(mvgpu_ctx *c, const uint8_t *mask) {
   if (!mask) { c->have_mov = false; return 0; }
   TRY(c->mov_in.ensure(c->lnv));
   if (c->lnv) {                                // on the context's stream, behind any run still reading mov_in
-    const uint8_t *src = mask;
-    if (w != Where::Device) {
-      CK(cudaMemcpyAsync(c->mov_in.p, mask, c->lnv, cudaMemcpyHostToDevice, c->stream));
-      src = c->mov_in.p;
-    }
+    const uint8_t *src;
+    TRY(to_device(c, mask, c->lnv, w, c->mov_in, src));
     // kept as 0 / 1, the form mvgpu_get_movable returns (the run's kernels read any nonzero byte as movable)
     k_mask01<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(src, c->lnv, c->mov_in.p);
     CK(cudaGetLastError());
@@ -2649,8 +2672,8 @@ int mvgpu_get_movable(mvgpu_ctx *c, uint8_t *out) {
   // on the context's stream: the run leaves k_movable_out queued behind its end event (and c->stream does not
   // synchronise with the legacy default stream)
   if (c->mov_out_valid || c->have_mov)
-    CK(cudaMemcpyAsync(out, c->mov_out_valid ? c->mov_out.p : c->mov_in.p, c->lnv, cudaMemcpyDefault, c->stream));
-  else if (w == Where::Device)
+    return to_caller(c, c->mov_out_valid ? c->mov_out.p : c->mov_in.p, c->lnv, w, out);
+  if (w == Where::Device)
     CK(cudaMemsetAsync(out, 1, (size_t)c->lnv, c->stream));
   else
     memset(out, 1, (size_t)c->lnv);
@@ -2717,8 +2740,7 @@ int mvgpu_get_community_matches(mvgpu_ctx *c, int64_t *size, int64_t *best, int6
   const std::string err = locate_all(c, 4, arr, names, w);
   if (!err.empty()) return fail("mvgpu_get_community_matches: " + err);
   for (int k = 0; k < 4; k++)
-    if (dst[k] && n) CK(cudaMemcpyAsync(dst[k], c->cmp_match.p + k * n, sizeof(long long) * n, cudaMemcpyDefault, c->stream));
-  CK(cudaStreamSynchronize(c->stream));
+    if (dst[k]) TRY(to_caller(c, c->cmp_match.p + k * n, sizeof(long long) * n, w[k], dst[k]));
   return 0;
 }
 
@@ -2732,10 +2754,9 @@ int mvgpu_get_community_stats(mvgpu_ctx *c, int64_t *size, double *volume, doubl
   Where w[3];
   const std::string err = locate_all(c, 3, arr, names, w);
   if (!err.empty()) return fail("mvgpu_get_community_stats: " + err);
-  if (size && n) CK(cudaMemcpyAsync(size, c->q_size.p, sizeof(long long) * n, cudaMemcpyDefault, c->stream));
-  if (volume && n) CK(cudaMemcpyAsync(volume, c->q_vol.p, sizeof(double) * n, cudaMemcpyDefault, c->stream));
-  if (internal && n) CK(cudaMemcpyAsync(internal, c->q_internal.p, sizeof(double) * n, cudaMemcpyDefault, c->stream));
-  CK(cudaStreamSynchronize(c->stream));
+  if (size) TRY(to_caller(c, c->q_size.p, sizeof(long long) * n, w[0], size));
+  if (volume) TRY(to_caller(c, c->q_vol.p, sizeof(double) * n, w[1], volume));
+  if (internal) TRY(to_caller(c, c->q_internal.p, sizeof(double) * n, w[2], internal));
   return 0;
 }
 
@@ -2777,32 +2798,7 @@ int mvgpu_get_communities(mvgpu_ctx *c, int64_t *out) {
   if (!err.empty()) return fail("mvgpu_get_communities: " + err);
   if (c->lnv == 0) return 0;
   TRY(final_in_caller_order(c));
-  // device and pinned destinations are written by put_ids; pageable ones are copied through the pinned bounce buffers
-  // in chunks (full PCIe rate instead of the driver's staged pageable path)
-  if (w != Where::Pageable) return put_ids(c, c->final_orig.p, out, w);
-  TRY(c->wide.ensure(c->lnv));
-  k_widen<<<grid_for(c->lnv, 256, c->num_sms), 256, 0, c->stream>>>(c->final_orig.p, c->lnv, c->wide.p);
-  const long long CH = kBounce;
-  TRY(bounce_buffers(c));
-  struct { long long off, n; } pend[2] = {{0, 0}, {0, 0}};
-  cudaEvent_t ev[2] = {get_event(c, 0), get_event(c, 1)};
-  long long off = 0;
-  for (int k = 0; off < c->lnv || pend[0].n || pend[1].n; k++) {
-    const int b = k & 1;
-    if (pend[b].n) {                                               // drain this buffer (its DMA was issued two steps ago,
-      CK(cudaEventSynchronize(ev[b]));                             //  the other buffer's DMA is in flight meanwhile)
-      memcpy(out + pend[b].off, c->h_bounce[b], sizeof(long long) * pend[b].n);
-      pend[b].n = 0;
-    }
-    if (off < c->lnv) {
-      const long long n = std::min<long long>(CH, c->lnv - off);
-      CK(cudaMemcpyAsync(c->h_bounce[b], c->wide.p + off, sizeof(long long) * n, cudaMemcpyDeviceToHost, c->stream));
-      CK(cudaEventRecord(ev[b], c->stream));
-      pend[b].off = off; pend[b].n = n;
-      off += n;
-    }
-  }
-  return 0;
+  return put_ids(c, c->final_orig.p, out, w);
 }
 
 // one option; a refusal changes nothing

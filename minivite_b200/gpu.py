@@ -460,7 +460,9 @@ class LouvainGPU:
 
     def communities(self, out=None, device=False):
         """currComm of this rank's vertices (global community ids).  `out`: optional preallocated int64 array
-        (a pinned one is filled at full PCIe rate).  device=True: a torch tensor on the context's device instead."""
+        (pinned or pageable: a pinned one is filled by one copy, a pageable one in chunks through the library's pinned
+        bounce buffers, so neither takes the driver's staged pageable copy).  device=True: a torch tensor on the context's
+        device instead."""
         if device:
             assert out is None, "device=True allocates its own tensor"
             (t,), (p,) = _outputs(True, self.device, self.lnv, ("i8",))

@@ -377,6 +377,41 @@ def test_pinned_and_pageable_host_arrays_take_the_host_form(gpu):
         R.close()
 
 
+# ---- 6. arrays larger than one bounce buffer ---------------------------------------------------------------------------------
+def test_arrays_larger_than_one_bounce_buffer(gpu):
+    """9 000 000 int64 ids are 72 MB: two full 32 MB chunks and a ragged tail through the pinned bounce buffers, both
+    ways.  The split and the warm start give the device form's bits from every input form, into every output form."""
+    from minivite_b200 import gpu as G
+    nv = 9_000_000
+    assert 2 * (4 << 20) < nv < 3 * (4 << 20)
+    g = G.LouvainGPU(0, 0, 1)
+    try:
+        g.generate_rgg(nv)
+        g.louvain()
+        pinned = put(np.zeros(nv, np.int64), "pinned")
+
+        def communities():
+            """The run's result, read into pageable, pinned and device memory: one array."""
+            dev = get(g.communities(device=True))
+            assert np.array_equal(g.communities(), dev) and np.array_equal(g.communities(out=pinned), dev)
+            return dev
+
+        X = communities()
+        split = {(f, d): g.split_communities(put(X, f), device=d) for f in FORMS for d in (False, True)}
+        Y, rep = get(split["torch", True][0]), strip(split["torch", True][1])
+        for key, (y, r) in split.items():
+            assert np.array_equal(get(y), Y) and strip(r) == rep, key
+        g.set_option("stop_after", 1)
+        warm = {}
+        for f in FORMS:
+            g.set_initial_communities(put(Y, f))
+            warm[f] = (g.louvain(), communities())
+        for f in FORMS:
+            assert warm[f][0] == warm["torch"][0] and np.array_equal(warm[f][1], warm["torch"][1]), f
+    finally:
+        g.close()
+
+
 # ---- one process per rank (CUDA IPC between processes), device inputs and outputs -----------------------------------------
 def _ipc_worker(rank, world, port, out_dir):
     os.environ.update(RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1",
